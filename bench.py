@@ -1,12 +1,18 @@
 #!/usr/bin/env python
-"""bench.py — Cambrian-1 training-step throughput on N x B200 (BASELINE.json metric) + roofline + CPU baseline.
+"""bench.py — Cambrian-1 training-step throughput on N x H100 (BASELINE.json metric) + roofline + CPU baseline.
 
-    python bench.py --gpus N --steps K --warmup W                    # this framework (hand-written sm_100a kernels)
+    python bench.py --gpus N --steps K --warmup W                    # this framework (hand-written sm_90a kernels)
     python bench.py --impl reference --gpus N --steps K --warmup W   # the reference algorithm on the host cores
-    python bench.py --config {8b-ddp,7b-clip-mlp,13b-zero2} ...      # BASELINE.json configs 3 (default), 2, 4
+    python bench.py --config {8b-ddp,7b-clip-mlp,13b-zero2} ...      # BASELINE.json configs 3, 2, 4
     python bench.py --config 8b-release                              # the released 8B recipe's towers / grids (not a BASELINE config)
+    python bench.py ... --dump-outputs DIR                           # also write the last timed step's results as .npy
 
 Workloads (SURVEY.md §8d):
+  3b-ddp       the default: the 8b-ddp vision stack (four towers, SVA connector + 10 in-LLM SVA layers) on a
+               Llama-3.2-3B-shaped decoder (28 L, H 3072, 24/8 heads x 128, FFN 8192, vocab 128256), seq 2048, per-layer
+               recompute: the largest Cambrian training step whose fp32 master weights + AdamW state (16 B per trainable
+               parameter, ~62 GB) fit one 80 GB H100.  The 8B / 7B decoders need ~128 / ~112 GB of such state per GPU
+               under DDP, so 8b-ddp and 7b-clip-mlp run on GPUs with more memory than an H100 has.
   8b-ddp       config 3 — Llama-3-8B decoder (32 L, H 4096, 32/8 heads x 128, FFN 14336, vocab 128256), four towers
                (SigLIP-SO400M/14@384, CLIP ViT-L/14@336, DINOv2 ViT-L/14@336, ConvNeXt-XXL@1024 — each interpolated to 576
                tokens), SVA connector depth 3 + 10 in-LLM SVA layers (start 0, stride 3), image_position 91, 576 visual
@@ -57,6 +63,9 @@ LLMS = {
     "vicuna-13b": dict(hidden_size=5120, intermediate_size=13824, num_hidden_layers=40, num_attention_heads=40,
                        num_key_value_heads=40, vocab_size=32000, max_position_embeddings=4096, rope_theta=10000.0,
                        rms_norm_eps=1e-5),
+    "llama3.2-3b": dict(hidden_size=3072, intermediate_size=8192, num_hidden_layers=28, num_attention_heads=24,
+                        num_key_value_heads=8, vocab_size=128256, max_position_embeddings=8192, rope_theta=500000.0,
+                        rms_norm_eps=1e-5),
     "small": dict(hidden_size=1024, intermediate_size=2048, num_hidden_layers=4, num_attention_heads=8,
                   num_key_value_heads=2, vocab_size=8192, max_position_embeddings=8192, rope_theta=500000.0,
                   rms_norm_eps=1e-5),
@@ -66,6 +75,12 @@ FOUR_TOWERS = ["siglip/CLIP-ViT-SO400M-14-384", "openai/clip-vit-large-patch14-3
 RELEASE_TOWERS = ["siglip/CLIP-ViT-SO400M-14-384", "openai/clip-vit-large-patch14-336", "facebook/dinov2-giant-res378",
                   "clip-convnext-XXL-multi-stage"]
 CONFIGS = {
+    "3b-ddp": dict(llm="llama3.2-3b", towers=FOUR_TOWERS, res=[384, 336, 336, 1024], sva=True, stride=3, n_sva=10,
+                   image_position=91, seq=2048, micro_batch=4, zero=0, recompute=1, baseline_config=None,
+                   tower_tf=sum(TOWER_TF.values()),
+                   workload="Cambrian-1 train step on one H100: 4 towers (SigLIP-SO400M@384, CLIP-L@336, DINOv2-L@336, "
+                            "ConvNeXt-XXL@1024) -> SVA (3 + 10 layers) -> Llama-3.2-3B-shaped decoder, 576 vis-tok, seq 2048, "
+                            "per-layer recompute"),
     "8b-release": dict(llm="llama3-8b", towers=RELEASE_TOWERS, res=[384, 336, 378, 1024], token_lens=[576, 576, 576, 9216],
                        sva=True, stride=3, n_sva=10, image_position=91, seq=2048, micro_batch=4, zero=0, recompute=1,
                        baseline_config=None, tower_tf=sum(TOWER_TF_RELEASE.values()), aux_tf=0.136,
@@ -326,7 +341,7 @@ class KernelTimer:
                 f"act={k[4]} bias={int(k[5])} res={int(k[6])}" for k, (fl, ms, n) in rows]
 
     def dominant(self):
-        """The fused gate/up + SwiGLU GEMM launches alone (the kernel `roofline.traffic` was captured on): per-launch
+        """The fused gate/up + SwiGLU GEMM launches alone: per-launch
         algorithmic FLOP / average CUDA-event duration."""
         fl = ms = 0.0
         n = 0
@@ -341,7 +356,7 @@ class KernelTimer:
             shape = (rec[0], rec[1])
         if n == 0 or ms <= 0:
             return None
-        return dict(kernel="gemm_bf16_tcgen05_2cta<256,0,0,swiglu_pair> (cb_gemm_swiglu_bf16)",
+        return dict(kernel="gemm_bf16_wgmma<128,0,0,swiglu_pair> (cb_gemm_swiglu_bf16)",
                     shape=f"M={shape[0][0]} 2F={shape[0][1]} K={shape[1]}", launches_timed=n,
                     flop_per_launch=fl / n, avg_launch_ms=ms / n, achieved=fl / (ms / 1000.0) / 1e12)
 
@@ -360,19 +375,9 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", 1400.0), d.get("bf16_tflops", 1590.0), "measured"
-    return 6650.0, 1400.0, 1590.0, "fallback"
-
-
-def ncu_traffic(key):
-    """DRAM read+write bytes of ONE launch, from the committed ncu artefact index (profiles/roofline_traffic.json: each
-    entry names the `ncu --set full` summary it was read from).  None when the kernel has no capture."""
-    try:
-        d = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json")))
-        e = d.get(key)
-        return (e["dram_bytes"], e["source"], e.get("algorithmic_bytes")) if e else (None, None, None)
-    except Exception:
-        return None, None, None
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops_sustained", 989.0), d.get("bf16_tflops", 989.0), "measured"
+    # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s — a bound, not a measured rate
+    return 3350.0, 989.0, 989.0, "H100 SXM data sheet"
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -401,6 +406,26 @@ def run_reference(args, rank, world):
     print(json.dumps(line))
 
 
+DUMP_PER_TENSOR = 4096
+
+
+def dump_outputs(out_dir, loss, model):
+    """What the timed step hands back to its caller: the loss, and the trainable parameters it updated (a fixed, seeded
+    sample of DUMP_PER_TENSOR elements per tensor, in named_parameters() order; ~5 MB for 3b-ddp)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float(loss.detach())], dtype=np.float32))
+    g = torch.Generator().manual_seed(0)
+    parts = []
+    for _, p in model.named_parameters():
+        if not p.requires_grad:
+            continue
+        flat = p.detach().reshape(-1)
+        idx = torch.randint(0, flat.numel(), (min(DUMP_PER_TENSOR, flat.numel()),), generator=g)
+        parts.append(flat[idx.to(flat.device)].float().cpu())
+    np.save(os.path.join(out_dir, "params_sample.npy"), torch.cat(parts).numpy())
+
+
 # ------------------------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -408,7 +433,7 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--config", default=os.environ.get("CB_BENCH_CONFIG", "8b-ddp"), choices=sorted(CONFIGS))
+    ap.add_argument("--config", default=os.environ.get("CB_BENCH_CONFIG", "3b-ddp"), choices=sorted(CONFIGS))
     ap.add_argument("--micro-batch", type=int, default=int(os.environ.get("CB_MICRO_BATCH", "0")))
     ap.add_argument("--seq", type=int, default=0)
     ap.add_argument("--recompute", type=int, default=int(os.environ.get("CB_RECOMPUTE", "-1")),
@@ -418,6 +443,9 @@ def main():
     ap.add_argument("--bucket-mb", type=float, default=float(os.environ.get("CB_BUCKET_MB", "256")))
     ap.add_argument("--small", action="store_true", help="tiny shapes for a functional check (not a valid bench)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's loss and a fixed seeded sample of the updated "
+                         "trainable parameters to DIR as float32 .npy files (compare two builds output for output)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -431,8 +459,8 @@ def main():
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
-        # NCCL's own tuner picks the LL protocol for the 256 MB gradient buckets on this box (timeline:
-        # ncclDevKernel_AllReduce_Sum_bf16_RING_LL); Simple measured +1 % at N = 8 (profiles/r02_bench_e_n8*.json)
+        # NCCL's own tuner picks the LL protocol for the 256 MB gradient buckets; Simple streams large buckets at least as
+        # well (measured on an earlier 8-GPU node; not re-measured on H100)
         os.environ.setdefault("NCCL_PROTO", "Simple")
         dist.init_process_group("nccl", device_id=dev)
     from cambrian_b200 import _lib, ops
@@ -475,9 +503,9 @@ def main():
     # off with CB_BENCH_HINTS=0: the model then counts labels / locates the image span on the device — still no host sync —
     # and the fused loss processes every row like the reference).
     hints = os.environ.get("CB_BENCH_HINTS", "1") != "0"
-    host_batches = [make_host_batch(cfg, B, S, 1000 * rank + i, res, hints) for i in range(2)]
-    dev_batch, h2d_bytes = to_device(host_batches[0], dev)
-    label_ranges = host_batches[0].get("label_ranges")
+    host_batch = make_host_batch(cfg, B, S, 1000 * rank, res, hints)
+    dev_batch, h2d_bytes = to_device(host_batch, dev)
+    label_ranges = host_batch.get("label_ranges")
     torch.cuda.synchronize()
 
     def step_resident():
@@ -486,14 +514,6 @@ def main():
         out.loss.backward()
         engine.step()
         return out.loss
-
-    def step_e2e(i):
-        db, _ = to_device(host_batches[i % 2], dev)
-        engine.zero_grad()
-        out = model(**db)
-        out.loss.backward()
-        engine.step()
-        return float(out.loss.detach().item())  # device -> host read of the step's result
 
     def barrier():
         if world > 1:
@@ -511,7 +531,7 @@ def main():
     timer.wrap(ops)
     sampler = ClockSampler(local_rank)
     sampler.start()
-    # ---- timed region 1: inputs resident in HBM
+    # ---- timed region: inputs resident in HBM
     barrier()
     timer.enabled = True
     l0 = lib.cb_launch_count()
@@ -527,22 +547,14 @@ def main():
     timer.enabled = False
     launches = (lib.cb_launch_count() - l0) // args.steps
     ms = e0.elapsed_time(e1)
-    # ---- timed region 2: end to end through the public API with host buffers
-    barrier()
-    e2, e3 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e2.record()
-    for i in range(args.steps):
-        lv = step_e2e(i)
-    engine.wait_for_params()
-    e3.record()
-    barrier()
-    ms_e2e = e2.elapsed_time(e3)
     sampler.stop_flag = True
     sampler.join(timeout=3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, model)
     if world > 1:
-        t = torch.tensor([ms, ms_e2e], device=dev)
+        t = torch.tensor([ms], device=dev)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        ms, ms_e2e = float(t[0]), float(t[1])
+        ms = float(t[0])
     if rank != 0:
         if world > 1:
             dist.destroy_process_group()
@@ -550,7 +562,6 @@ def main():
 
     ms_step = ms / args.steps
     value = world * B / (ms_step / 1000.0)
-    e2e_value = world * B / (ms_e2e / args.steps / 1000.0)
     hbm_peak, tf_sustained, tf_burst, peak_src = peaks()
     agg = timer.totals()
     if os.environ.get("CB_BENCH_SHAPES"):
@@ -559,8 +570,8 @@ def main():
     if "gemm" in agg:
         fl, tms, n = agg["gemm"]
         ach = fl / (tms / 1000.0) / 1e12
-        roof = dict(bound="tensor", kernel="gemm_bf16_tcgen05", achieved=ach, peak=tf_sustained, unit="TFLOP/s",
-                    frac=ach / tf_sustained, traffic=None, launches_timed=n, share_of_step=tms / ms,
+        roof = dict(bound="tensor", kernel="gemm_bf16_wgmma", achieved=ach, peak=tf_sustained, unit="TFLOP/s",
+                    frac=ach / tf_sustained, launches_timed=n, share_of_step=tms / ms,
                     peak_source=f"{peak_src} bf16_tflops_sustained (kernel timed inside a long step)",
                     scope="every GEMM launched on the step's main stream (connector + SVA + decoder + loss, fwd and bwd); the "
                           "frozen towers run concurrently on four side streams where per-launch event times overlap and are "
@@ -571,12 +582,6 @@ def main():
             if dom is not None:
                 dom["frac"] = dom["achieved"] / tf_sustained
                 roof["dominant_launch"] = dom
-                key = "gemm_swiglu_" + dom["shape"].replace(" ", "_").replace("=", "")
-                tr, src, alg = ncu_traffic(key)
-                roof["traffic"] = tr
-                roof["traffic_note"] = (f"dram read+write bytes of ONE launch of the dominant kernel ({dom['shape']}), read "
-                                        f"from {src}; algorithmic {alg} B" if tr else
-                                        f"no committed ncu capture for {key} (profiles/roofline_traffic.json)")
         except Exception as exc:  # never let optional reporting break the bench line
             roof["dominant_launch"] = {"error": str(exc)}
 
@@ -621,12 +626,9 @@ def main():
             roof_sva[tag] = dict(achieved=ach, frac=ach / hbm_peak, algorithmic_bytes_per_launch=byts,
                                  mb_per_sample_per_layer=byts / Bq / 1e6)
             del qq, ks, vs
-        tr, src, alg = ncu_traffic("sva_window_attn_fwd_b32_576x4")
         roof_sva.update(bound="hbm", kernel="sva_window_attn_fwd", peak=hbm_peak, unit="GB/s",
                         achieved=roof_sva["baseline_grids_576x4"]["achieved"],
-                        frac=roof_sva["baseline_grids_576x4"]["frac"], traffic=tr, peak_source=f"{peak_src} hbm_gbs",
-                        traffic_note=f"ncu dram bytes of one batch-32 launch on the BASELINE grids, from {src} (algorithmic "
-                                     f"{alg} B)" if tr else "no committed ncu capture")
+                        frac=roof_sva["baseline_grids_576x4"]["frac"], peak_source=f"{peak_src} hbm_gbs")
         if "sva_fwd" in agg:
             by, tms, n = agg["sva_fwd"]
             roof_sva["in_step_achieved"] = by / (tms / 1000.0) / 1e9  # B=4 inputs (38 MB) are L2-resident in the step
@@ -655,7 +657,7 @@ def main():
                 gpu_launches=int(launches), host_enqueue_ms_per_step=round(host_enqueue_ms, 1), loss=float(loss.detach()),
                 peak_mem_gb=round(torch.cuda.max_memory_allocated() / 2 ** 30, 1),
                 peak_reserved_gb=round(torch.cuda.max_memory_reserved() / 2 ** 30, 1),
-                e2e=dict(value=e2e_value, unit=UNIT, h2d_bytes_per_step=int(h2d_bytes), d2h_bytes_per_step=4),
+                h2d_bytes_per_batch=int(h2d_bytes),
                 clocks=sampler.summary(), roofline=roof, roofline_sva=roof_sva, roofline_attn=roof_attn,
                 roofline_adamw=roof_adamw,
                 model_tflops_per_gpu=(model_tf / world) if model_tf else None,

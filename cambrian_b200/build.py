@@ -1,7 +1,7 @@
-"""In-tree build of libcambrian_b200.so (sm_100a only).
+"""In-tree build of libcambrian_b200.so (sm_90a, H100, only).
 
 `python -m cambrian_b200.build` cross-compiles every csrc/*.cu with nvcc (no GPU needed) and links one
-shared library next to this file, where the ctypes loader (`_lib.py`) and `gpurun` snapshots find it.
+shared library next to this file, where the ctypes loader (`_lib.py`) finds it.
 """
 from __future__ import annotations
 
@@ -17,7 +17,7 @@ OBJ = HERE / "csrc" / "_obj"
 LIB = HERE / "libcambrian_b200.so"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-O3", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3", "-lineinfo",
     "-Xcompiler", "-fPIC", "--use_fast_math", "-Xptxas", "-v",
 ]
 # --use_fast_math would change erff/expf/division accuracy in the numerics-critical kernels; keep IEEE
@@ -51,7 +51,7 @@ def build(verbose: bool = True) -> Path:
     with cf.ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(lambda s: _compile(s, verbose), srcs))
     if not LIB.exists() or any(o.stat().st_mtime > LIB.stat().st_mtime for o in objs):
-        cmd = [NVCC, "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [NVCC, "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -8,7 +8,7 @@ the unchanged `PreTrainedModel.from_pretrained`.  This file adds the three refer
     (`safe_save_model_for_hf_trainer`, train_fsdp.py:249-283; key filter :255);
   * `load_mm_projector` — the `mm_projector.bin` overlay on top of a base LLM (model/builder.py:107-114) and the
     `pretrain_mm_mlp_adapter` path of `initialize_vision_modules` (cambrian_arch.py:183-200, strict per sub-module);
-  * `load_pretrained_model` — the loader the eval / serve harness calls (model/builder.py:29-175), bf16 on one B200.
+  * `load_pretrained_model` — the loader the eval / serve harness calls (model/builder.py:29-175), bf16 on one GPU.
     LoRA merging and 4/8-bit quantised loading are outside the hot path and raise NotImplementedError.
 """
 from __future__ import annotations
@@ -75,7 +75,7 @@ def load_pretrained_model(model_path, model_base=None, model_name="cambrian", lo
 
     from .model.language_model.cambrian_llama import CambrianLlamaForCausalLM
     if load_8bit or load_4bit:
-        raise NotImplementedError("bitsandbytes-quantised loading is not part of the B200 path (bf16 only)")
+        raise NotImplementedError("bitsandbytes-quantised loading is not part of this path (bf16 only)")
     if "lora" in model_name.lower():
         raise NotImplementedError("LoRA merging (builder.py:56-92) is outside the hot path: merge with the reference tools first")
     if "mistral" in model_name.lower() or "phi3" in model_name.lower():

@@ -40,7 +40,7 @@ class SymmetricAllReduce:
         self.multicast = mc if use_multicast else 0
         # 128-thread CTAs that share SMs with the GEMM CTAs: one per SM keeps enough switch round trips in flight at any
         # world size (each GPU moves 1/world of a bucket through its own loads / stores)
-        self.ctas = int(ctas) if ctas else min(148, _lib.load().cb_sm_count())
+        self.ctas = int(ctas) if ctas else _lib.load().cb_sm_count()
         self.epoch = 1
         dist.barrier(group=self.group)                   # every rank's flags are zero before anyone raises one
 

@@ -24,10 +24,10 @@ long long launch_count() { return g_launches.load(std::memory_order_relaxed); }
 int device_sm_count() {
   static int sms[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (sms[dev] == 0) {
     int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
     sms[dev] = v;
   }
   return sms[dev];
@@ -85,7 +85,6 @@ int cross_entropy_launch(void*, const long long*, float*, float*, long long, lon
 int adamw_launch(float*, float*, float*, const void*, void*, long long, float, float, float, float, float, int, float,
                  const float*, int, cudaStream_t);
 int sumsq_launch(const void*, long long, float*, float*, long long, int, cudaStream_t);
-int gemm_set_dynamic_scheduling(int);
 int gemv_bf16_launch(const void*, const void*, void*, int, int, int, long long, long long, long long, const void*, const void*,
                      long long, int, cudaStream_t);
 int allreduce_symm_launch(unsigned long long, const unsigned long long*, const unsigned long long*, long long, long long, int,
@@ -319,7 +318,6 @@ int cb_gemv_bf16(const void* x, const void* w, void* y, int M, int N, int K, int
                  const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream) {
   return cb::gemv_bf16_launch(x, w, y, M, N, K, ldx, ldw, ldy, bias, residual, ldr, out_fp32, ST(stream));
 }
-int cb_gemm_set_dynamic_scheduling(int on) { return cb::gemm_set_dynamic_scheduling(on); }
 int cb_sumsq_bf16(const void* g, int64_t n, float* acc, float* workspace, int64_t workspace_floats, int background,
                   void* stream) {
   return cb::sumsq_launch(g, n, acc, workspace, workspace_floats, background, ST(stream));

@@ -1,4 +1,4 @@
-// cambrian_b200 — tcgen05 flash attention (forward + backward) for sm_100a.
+// cambrian_b200 — wgmma flash attention (forward + backward) for sm_90a (H100).
 //
 // Covers the two softmax-attention shapes of the hot path (SURVEY.md §8a):
 //   * ViT towers (A1-A3): non-causal, head_dim 64 (CLIP, DINOv2) / 72 (SigLIP), 577 / 729 tokens, fwd only
@@ -8,17 +8,17 @@
 // Layout: q/k/v/o are addressed as (b, s, head, d) with arbitrary batch / row strides and heads packed along the
 // row, so the fused QKV GEMM output [B*S, (nh + 2 nkv) * hd] is consumed in place (no permute / contiguous).
 //
-// Forward (one CTA = 128 query rows of one head; 192 threads):
-//   warp 4  TMA producer : Q once, then K_j / V_j tiles through two mbarrier rings
-//   warp 5  MMA issuer   : S_j = Q K_j^T (tcgen05, fp32 in TMEM, double buffered), O += P_j V_j
-//   warps 0-3 softmax    : one thread per query row (TMEM lane == row: no shuffles), online softmax in the
-//                          log2 domain with lazy rescale of the TMEM-resident O, P_j written as bf16 into a
-//                          128B-swizzled smem tile that the PV MMA reads as its A operand.
-// Backward (one CTA = 128 keys of one KV head; loops over the query heads of the GQA group and the query tiles):
-//   S^T = K Q^T and dP^T = V dO^T in TMEM; threads (one per key row) form P^T (bf16, back into TMEM as the A
-//   operand of dV += P^T dO) and dS^T (bf16, smem: K-major A of dK += dS^T Q and MN-major A of dQ_i = dS K);
-//   dK / dV accumulate in TMEM over the whole loop, dQ partials are staged as fp32 tiles in the Q / dO stage the
-//   iteration just retired and reduce-added into global memory by TMA (cp.reduce.async.bulk.tensor .add).
+// Forward (one CTA = 128 query rows of one head; 288 threads):
+//   warp 8     TMA producer : Q once, then K_j / V_j tiles through an mbarrier ring
+//   warps 0-7  two consumer warpgroups of 64 query rows: S_j = Q K_j^T (wgmma, fp32 in registers), online softmax in
+//              the log2 domain (rows are spread over the 4 lanes of a quad), P_j re-packed in registers as the bf16
+//              A operand of O += P_j V_j (wgmma with A from registers, V read MN-major from shared memory).
+// Backward, two kernels so that every output element has exactly one writer (no atomics: bit-identical run to run):
+//   dK / dV: one CTA = 128 keys of one KV head, two warpgroups of 64 keys, looping over the query heads of the GQA group
+//     and the 64-row query tiles: S^T = K Q^T and dP^T = V dO^T in registers; P^T and dS^T are re-packed in registers as
+//     the A operands of dV += P^T dO and dK += dS^T Q.
+//   dQ: one CTA = 128 queries of one head (same layout as the forward), looping over 64-key tiles: S = Q K^T and
+//     dP = dO V^T in registers, dS re-packed as the A operand of dQ += dS K; dQ is stored once per element.
 #include "common.cuh"
 #include <cudaTypedefs.h>
 
@@ -41,15 +41,13 @@ struct AttnParams {
 template <int HDP>
 struct FwdCfg {
   static constexpr int ATOMS = (HDP + 63) / 64;
-  static constexpr int TILE = ATOMS * 16384;         // one [128 x hd] operand tile
+  static constexpr int TILE = ATOMS * 16384;         // one [128 x hd] operand tile, 64-column SWIZZLE_128B atoms
   static constexpr int STAGES = (HDP <= 64) ? 3 : 2;
-  static constexpr int P_BYTES = 32768;               // [128 x 128] bf16
-  static constexpr int SMEM = TILE * (1 + 2 * STAGES) + P_BYTES + 1024 + 256;
-  static constexpr int OCH = (HDP + 31) / 32;         // 32-column chunks of O
+  static constexpr int SMEM = TILE * (1 + 2 * STAGES) + 1024 + 256;
 };
 
 template <int HDP>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(288, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, AttnParams p) {
   using Cfg = FwdCfg<HDP>;
@@ -59,17 +57,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const uint32_t sQ = base;
   const uint32_t sK = sQ + Cfg::TILE;
   const uint32_t sV = sK + STAGES * Cfg::TILE;
-  const uint32_t sP = sV + STAGES * Cfg::TILE;
-  const uint32_t bars = sP + Cfg::P_BYTES;
+  const uint32_t bars = sV + STAGES * Cfg::TILE;
   const uint32_t q_full = bars;
   auto k_full = [&](int s) { return bars + 8u * (1 + s); };
-  auto k_empty = [&](int s) { return bars + 8u * (1 + STAGES + s); };
-  auto v_full = [&](int s) { return bars + 8u * (1 + 2 * STAGES + s); };
-  auto v_empty = [&](int s) { return bars + 8u * (1 + 3 * STAGES + s); };
-  auto s_full = [&](int s) { return bars + 8u * (1 + 4 * STAGES + s); };
-  const uint32_t p_full = bars + 8u * (3 + 4 * STAGES);
-  const uint32_t pv_done = bars + 8u * (4 + 4 * STAGES);
-  const uint32_t tmem_slot = bars + 8u * (5 + 4 * STAGES);
+  auto v_full = [&](int s) { return bars + 8u * (1 + STAGES + s); };
+  auto kv_empty = [&](int s) { return bars + 8u * (1 + 2 * STAGES + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q_tiles = (p.Sq + 127) / 128;
@@ -87,32 +79,21 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     if (n_tiles < 1) n_tiles = 1;
   }
 
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     mbar_init(q_full, 1);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(k_full(s), 1);
-      mbar_init(k_empty(s), 1);
       mbar_init(v_full(s), 1);
-      mbar_init(v_empty(s), 1);
+      mbar_init(kv_empty(s), 2);  // one arrive per consumer warpgroup
     }
-    mbar_init(s_full(0), 1);
-    mbar_init(s_full(1), 1);
-    mbar_init(p_full, 128);
-    mbar_init(pv_done, 1);
     mbar_fence_init();
   }
-  if (warp == 5) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem) : "r"(tmem_slot));
-  const uint32_t tS0 = tmem, tO = tmem + 256;
 
-  if (warp == 4) {
+  if (warp == 8) {
     // ================================ TMA producer ================================
     if (lane == 0) {
       mbar_arrive_expect_tx(q_full, Cfg::TILE);
@@ -121,12 +102,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       int st = 0;
       uint32_t ph = 0;
       for (int j = 0; j < n_tiles; ++j) {
-        mbar_wait(k_empty(st), ph ^ 1u);
+        mbar_wait(kv_empty(st), ph ^ 1u);
         mbar_arrive_expect_tx(k_full(st), Cfg::TILE);
 #pragma unroll
         for (int a = 0; a < Cfg::ATOMS; ++a)
           tma_load_4d(sK + st * Cfg::TILE + a * 16384, &tmK, k_full(st), a * 64, hk, j * 128, b);
-        mbar_wait(v_empty(st), ph ^ 1u);
         mbar_arrive_expect_tx(v_full(st), Cfg::TILE);
 #pragma unroll
         for (int a = 0; a < Cfg::ATOMS; ++a)
@@ -134,184 +114,116 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         if (++st == STAGES) { st = 0; ph ^= 1u; }
       }
     }
-  } else if (warp == 5) {
-    // ================================ MMA issuer ==================================
-    if (lane == 0) {
-      constexpr uint32_t idesc_qk = make_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, HDP, 0, 1);
-      auto issue_s = [&](int j, int st) {
-        const uint32_t kb = sK + st * Cfg::TILE;
+    return;
+  }
+
+  // ================================ consumer warpgroups ================================
+  const int wg = warp >> 2;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's rows: rloc and rloc + 8
+  const int cq = 2 * (lane & 3);                             // and columns 8 j + cq, + 1 of every 8-column block
+  const uint8_t* km = p.kmask ? p.kmask + (size_t)b * p.Skv : nullptr;
+  float o[HDP / 2];
 #pragma unroll
-        for (int kk = 0; kk < HDP / 16; ++kk) {
-          const uint32_t off = (kk >> 2) * 16384 + (kk & 3) * 32;
-          umma_ss(tS0 + (j & 1) * 128, make_smem_desc_sw128(sQ + off, 0, 1024),
-                  make_smem_desc_sw128(kb + off, 0, 1024), idesc_qk, kk ? 1u : 0u);
-        }
-        umma_commit(k_empty(st));
-        umma_commit(s_full(j & 1));
-      };
-      mbar_wait(q_full, 0);
-      int kst = 0; uint32_t kph = 0;
-      int vst = 0; uint32_t vph = 0;
-      mbar_wait(k_full(0), 0);
-      tc_fence_after();
-      issue_s(0, 0);
-      if (++kst == STAGES) { kst = 0; kph ^= 1u; }
-      for (int j = 0; j < n_tiles; ++j) {
-        if (j + 1 < n_tiles) {
-          mbar_wait(k_full(kst), kph);
-          tc_fence_after();
-          issue_s(j + 1, kst);
-          if (++kst == STAGES) { kst = 0; kph ^= 1u; }
-        }
-        mbar_wait(p_full, j & 1);
-        mbar_wait(v_full(vst), vph);
-        tc_fence_after();
-        const uint32_t vb = sV + vst * Cfg::TILE;
+  for (int i = 0; i < HDP / 2; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  mbar_wait(q_full, 0);
+  int st = 0;
+  uint32_t ph = 0;
+  for (int j = 0; j < n_tiles; ++j) {
+    const int k0 = j * 128;
+    float s[64];
+    mbar_wait(k_full(st), ph);
+    const uint32_t kb = sK + st * Cfg::TILE;
+    wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const uint32_t aoff = (kk >> 2) * 16384 + (kk & 3) * 32;
-          umma_ss(tO, make_smem_desc_sw128(sP + aoff, 0, 1024),
-                  make_smem_desc_sw128(vb + kk * 2048, 16384, 1024), idesc_pv, (j | kk) ? 1u : 0u);
+    for (int kk = 0; kk < HDP / 16; ++kk) {
+      const uint32_t off = (kk >> 2) * 16384 + (kk & 3) * 32;
+      WgmmaSS<128, 0, 0>::mma(s, make_smem_desc_sw128(sQ + wg * 8192 + off, 0, 1024),
+                              make_smem_desc_sw128(kb + off, 0, 1024), kk ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    // masking (keys past Skv, past the diagonal, padded keys) -> -inf; scores into the log2 domain
+    const bool full_tile = !km && k0 + 128 <= p.Skv && (!p.causal || k0 + 127 <= q0 + wg * 64 + coff);
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        float v = s[4 * jj + e] * p.scale_log2;
+        if (!full_tile) {
+          const int key = k0 + 8 * jj + cq + (e & 1);
+          const int qi = q0 + rloc + 8 * (e >> 1);
+          const bool ok = key < p.Skv && (!p.causal || key <= qi + coff) && (!km || km[key]);
+          v = ok ? v : -INFINITY;
         }
-        umma_commit(v_empty(vst));
-        umma_commit(pv_done);
-        if (++vst == STAGES) { vst = 0; vph ^= 1u; }
+        s[4 * jj + e] = v;
+        mx[e >> 1] = fmaxf(mx[e >> 1], v);
       }
     }
-  } else {
-    // ================================ softmax warps ===============================
-    const int row = warp * 32 + lane;  // TMEM lane == query row in the tile
-    const int qi = q0 + row;
-    const uint32_t lane_off = static_cast<uint32_t>(warp * 32) << 16;
-    float m_ref = 0.f, l = 0.f;
-    for (int j = 0; j < n_tiles; ++j) {
-      const int k0 = j * 128;
-      int kmax = p.Skv - k0;                                // keys beyond Skv
-      if (p.causal) kmax = min(kmax, qi + coff - k0 + 1);   // keys beyond the diagonal
-      // key-padding mask of this tile as 4 x 32 bits, built cooperatively (lane l owns keys 4l..4l+3)
-      uint32_t mw[4] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu};
-      if (p.kmask) {
-        const uint8_t* km = p.kmask + (size_t)b * p.Skv + k0;
-        uint32_t nib = 0;
+    float corr[2], mref[2];
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int kc = lane * 4 + e;
-          if (k0 + kc < p.Skv && km[kc]) nib |= 1u << e;
-        }
-        uint32_t v = nib << (4 * (lane & 7));
-        v |= __shfl_xor_sync(0xffffffffu, v, 1);
-        v |= __shfl_xor_sync(0xffffffffu, v, 2);
-        v |= __shfl_xor_sync(0xffffffffu, v, 4);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) mw[c] = __shfl_sync(0xffffffffu, v, 8 * c);
-      }
-      mbar_wait(s_full(j & 1), (j >> 1) & 1);
-      tc_fence_after();
-      const uint32_t tS = tS0 + (j & 1) * 128 + lane_off;
-      // one TMEM read of the whole 128-key row into registers
-      uint32_t sr[128];
-      tmem_ld32(tS, sr);
-      tmem_ld32(tS + 32, sr + 32);
-      tmem_ld32(tS + 64, sr + 64);
-      tmem_ld32(tS + 96, sr + 96);
-      tmem_ld_wait();
-      if (kmax < 128 || p.kmask) {  // branch-free masking: masked scores become -inf
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const int rem = kmax - c * 32;
-          uint32_t bits = rem >= 32 ? 0xffffffffu : (rem <= 0 ? 0u : ((1u << rem) - 1u));
-          bits &= mw[c];
-#pragma unroll
-          for (int e = 0; e < 32; ++e) sr[c * 32 + e] = ((bits >> e) & 1u) ? sr[c * 32 + e] : 0xff800000u;
-        }
-      }
-      float t0 = -INFINITY, t1 = -INFINITY, t2 = -INFINITY, t3 = -INFINITY;
-#pragma unroll
-      for (int e = 0; e < 128; e += 4) {
-        t0 = fmaxf(t0, __uint_as_float(sr[e]));
-        t1 = fmaxf(t1, __uint_as_float(sr[e + 1]));
-        t2 = fmaxf(t2, __uint_as_float(sr[e + 2]));
-        t3 = fmaxf(t3, __uint_as_float(sr[e + 3]));
-      }
-      float tmax = fmaxf(fmaxf(t0, t1), fmaxf(t2, t3)) * p.scale_log2;  // scale > 0 keeps ordering; -inf stays
-      // lazy rescale (log2 domain): only move the reference max when it grows by > 8 (p <= 256)
-      const bool grow = (j == 0) ? true : (tmax > m_ref + 8.f);
-      if (__any_sync(0xffffffffu, grow)) {
-        float m_new = (j == 0) ? tmax : fmaxf(m_ref, tmax);
-        if (m_new == -INFINITY) m_new = 0.f;
-        if (j > 0) {
-          const float corr = fast_exp2(m_ref - m_new);
-          l *= corr;
-          mbar_wait(pv_done, (j - 1) & 1);  // O accumulation of tile j-1 retired
-          tc_fence_after();
-#pragma unroll 1
-          for (int c = 0; c < Cfg::OCH; ++c) {
-            uint32_t r[32];
-            tmem_ld32(tO + lane_off + c * 32, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 32; ++e) r[e] = __float_as_uint(__uint_as_float(r[e]) * corr);
-            tmem_st32(tO + lane_off + c * 32, r);
-          }
-          tmem_st_wait();
-        }
-        m_ref = m_new;
-      } else if (j > 0) {
-        mbar_wait(pv_done, (j - 1) & 1);  // P smem tile free again
-      }
-      // p = exp2(s*scale - m_ref) (masked: exp2(-inf) = 0), row sum, bf16 P tile in the K-major SWIZZLE_128B layout
-      const float neg_m = -m_ref;
-      float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;
-#pragma unroll
-      for (int g = 0; g < 16; ++g) {  // 16-byte chunk index along the 128 keys
-        float pv[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) pv[e] = fast_exp2(fmaf(__uint_as_float(sr[g * 8 + e]), p.scale_log2, neg_m));
-        l0 += pv[0] + pv[4];
-        l1 += pv[1] + pv[5];
-        l2 += pv[2] + pv[6];
-        l3 += pv[3] + pv[7];
-        const uint32_t addr = sP + (g >> 3) * 16384 + row * 128 + (((g & 7) ^ (row & 7)) << 4);
-        const uint4 val = pack8(pv);
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(val.x), "r"(val.y), "r"(val.z),
-                     "r"(val.w) : "memory");
-      }
-      l += (l0 + l1) + (l2 + l3);
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(p_full);
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float m_new = fmaxf(m_run[r], mx[r]);
+      mref[r] = m_new == -INFINITY ? 0.f : m_new;  // fully masked so far: exp2(-inf - 0) = 0 keeps everything finite
+      corr[r] = fast_exp2(m_run[r] - mref[r]);
+      m_run[r] = m_new;
+      l_run[r] *= corr[r];
     }
-    // ---- epilogue: O / l -> bf16 -> HBM
-    mbar_wait(pv_done, (n_tiles - 1) & 1);
-    tc_fence_after();
+#pragma unroll
+    for (int jj = 0; jj < HDP / 8; ++jj) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[4 * jj + e] *= corr[e >> 1];
+    }
+    // P = exp2(s - m): row sums (per thread; the quad is summed once at the end) and the bf16 A fragments of P V
+    uint32_t pa[8][4];
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+      float pv[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        pv[e] = fast_exp2(s[4 * jj + e] - mref[e >> 1]);
+        l_run[e >> 1] += pv[e];
+      }
+      pa[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(pv[0], pv[1]);
+      pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(pv[2], pv[3]);
+    }
+    mbar_wait(v_full(st), ph);
+    const uint32_t vb = sV + st * Cfg::TILE;
+    reg_fence(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)
+      WgmmaRS<HDP, 1>::mma(o, pa[kk], make_smem_desc_sw128(vb + kk * 2048, 16384, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    if (wg_leader) mbar_arrive(kv_empty(st));
+    if (++st == STAGES) { st = 0; ph ^= 1u; }
+  }
+  // ---- epilogue: O / l -> bf16 -> HBM
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    float l = l_run[r];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const int qi = q0 + rloc + 8 * r;
+    if (qi >= p.Sq) continue;
     const float inv = l > 0.f ? 1.f / l : 0.f;
     bf16* op = p.o + (long long)b * p.o_bs + (long long)qi * p.o_ss + (long long)h * p.hd;
-#pragma unroll 1
-    for (int c = 0; c < Cfg::OCH; ++c) {
-      uint32_t r[32];
-      tmem_ld32(tO + lane_off + c * 32, r);
-      tmem_ld_wait();
-      if (qi < p.Sq) {
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const int d0 = c * 32 + u * 8;
-          if (d0 < p.hd) {
-            float f[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(r[u * 8 + e]) * inv;
-            *reinterpret_cast<uint4*>(op + d0) = pack8(f);
-          }
-        }
-      }
+    for (int jj = 0; jj < HDP / 8; ++jj) {
+      const int d = 8 * jj + cq;
+      if (d < p.hd)
+        *reinterpret_cast<__nv_bfloat162*>(op + d) = __floats2bfloat162_rn(o[4 * jj + 2 * r] * inv, o[4 * jj + 2 * r + 1] * inv);
     }
-    if (p.lse && qi < p.Sq)
-      p.lse[((long long)b * p.nh + h) * p.Sq + qi] = l > 0.f ? m_ref + log2f(l) : INFINITY;
+    if (p.lse && (lane & 3) == 0)
+      p.lse[((long long)b * p.nh + h) * p.Sq + qi] = l > 0.f ? m_run[r] + log2f(l) : INFINITY;
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 5) tmem_dealloc(tmem, 512);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -352,7 +264,7 @@ __global__ void attn_delta_kernel(const bf16* __restrict__ o, const bf16* __rest
 }
 
 struct AttnBwdParams {
-  float* dq_acc;            // [B, Sq, nh, hd] fp32, zero-initialised by the caller; holds sum of dS K (unscaled)
+  float* dq_acc;            // [B, Sq, nh, hd] fp32: receives dS K (unscaled), every element written once
   bf16* dk;                 // (b, s, kv head, d) with strides below
   bf16* dv;
   long long dk_bs, dk_ss, dv_bs, dv_ss;
@@ -365,329 +277,323 @@ struct AttnBwdParams {
 
 template <int HDP>
 struct BwdCfg {
-  static constexpr int ATOMS = (HDP + 63) / 64;
-  static constexpr int TILE = ATOMS * 16384;
-  static constexpr int DS_BYTES = 32768;
-  static constexpr int SMEM = TILE * 6 + DS_BYTES + 1024 + 1024 /*lse+delta*/ + 256;
-  static constexpr int OCH = (HDP + 31) / 32;
+  static constexpr int ATOMS = HDP / 64;
+  static constexpr int KTILE = ATOMS * 16384;  // [128 keys x hd]
+  static constexpr int QTILE = ATOMS * 8192;   // [64 queries x hd]
+  static constexpr int SMEM = 2 * KTILE + 4 * QTILE + 1024 + 256;
 };
 
 template <int HDP>
-__global__ void __launch_bounds__(320, 1)
+__global__ void __launch_bounds__(256, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
-                const __grid_constant__ CUtensorMap tmdQ, AttnBwdParams p) {
+                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, AttnBwdParams p) {
   using Cfg = BwdCfg<HDP>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sK = base;
-  const uint32_t sV = sK + Cfg::TILE;
-  const uint32_t sQ = sV + Cfg::TILE;        // 2 stages
-  const uint32_t sdO = sQ + 2 * Cfg::TILE;   // 2 stages
-  const uint32_t sdS = sdO + 2 * Cfg::TILE;  // [128 kv x 128 q] bf16, K-major over q
-  const uint32_t sStat = sdS + Cfg::DS_BYTES;  // float lse[128], delta[128]
-  const uint32_t bars = sStat + 1024;
+  const uint32_t sV = sK + Cfg::KTILE;
+  const uint32_t sQ = sV + Cfg::KTILE;       // 2 stages
+  const uint32_t sdO = sQ + 2 * Cfg::QTILE;  // 2 stages
+  const uint32_t bars = sdO + 2 * Cfg::QTILE;
   const uint32_t kv_full = bars;
   auto qd_full = [&](int s) { return bars + 8u * (1 + s); };
-  auto qd_empty = [&](int s) { return bars + 8u * (3 + s); };
-  const uint32_t sdp_full = bars + 8u * 5;   // S^T and dP^T ready in TMEM
-  const uint32_t pds_full = bars + 8u * 6;   // P^T (TMEM) and dS^T (smem) written by the 128 threads
-  const uint32_t dq_full = bars + 8u * 7;    // dQ partial ready in TMEM (also: dV/dK MMAs of this iteration retired)
-  const uint32_t dq_done = bars + 8u * 8;    // dQ partial read out by the 128 threads
-  const uint32_t dq_staged = bars + 8u * 9;  // fp32 dQ partial staged in this iteration's (retired) Q / dO stage
-  const uint32_t tmem_slot = bars + 8u * 10;
-  float* stat = reinterpret_cast<float*>(smem_raw + (sStat - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int jt = blockIdx.x, g = blockIdx.y, b = blockIdx.z;
   const int G = p.nh / p.nkv;
   const int k0 = jt * 128;
-  const int q_tiles = (p.Sq + 127) / 128;
+  const int q_tiles = (p.Sq + 63) / 64;
   const int coff = p.Skv - p.Sq;
   // causal: query i attends key k iff k <= i + coff  ->  first query tile that can see key k0
   int i_begin = 0;
   if (p.causal) {
     const int first_q = k0 - coff;
-    i_begin = first_q > 0 ? first_q / 128 : 0;
+    i_begin = first_q > 0 ? first_q / 64 : 0;
   }
   const int n_i = q_tiles > i_begin ? q_tiles - i_begin : 0;
   const int n_iter = n_i * G;
 
-  if (warp == 4 && lane == 0) {
+  auto load_qd = [&](int it) {
+    const int st = it & 1;
+    const int h = g * G + it / n_i;
+    const int qi0 = (i_begin + it % n_i) * 64;
+    mbar_arrive_expect_tx(qd_full(st), 2 * Cfg::QTILE);
+#pragma unroll
+    for (int a = 0; a < Cfg::ATOMS; ++a) {
+      tma_load_4d(sQ + st * Cfg::QTILE + a * 8192, &tmQ, qd_full(st), a * 64, h, qi0, b);
+      tma_load_4d(sdO + st * Cfg::QTILE + a * 8192, &tmdO, qd_full(st), a * 64, h, qi0, b);
+    }
+  };
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     tma_prefetch_desc(&tmdO);
-    tma_prefetch_desc(&tmdQ);
     mbar_init(kv_full, 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(qd_full(s), 1);
-      mbar_init(qd_empty(s), 1);
+    mbar_init(qd_full(0), 1);
+    mbar_init(qd_full(1), 1);
+    mbar_fence_init();
+    mbar_arrive_expect_tx(kv_full, 2 * Cfg::KTILE);
+#pragma unroll
+    for (int a = 0; a < Cfg::ATOMS; ++a) {
+      tma_load_4d(sK + a * 16384, &tmK, kv_full, a * 64, g, k0, b);
+      tma_load_4d(sV + a * 16384, &tmV, kv_full, a * 64, g, k0, b);
     }
-    mbar_init(sdp_full, 1);
-    mbar_init(pds_full, 256);
-    mbar_init(dq_full, 1);
-    mbar_init(dq_done, 256);
-    mbar_init(dq_staged, 256);
+    if (n_iter > 0) load_qd(0);
+    if (n_iter > 1) load_qd(1);
+  }
+  __syncthreads();
+
+  const int wg = warp >> 2;
+  const int kr = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's key rows kr, kr + 8 (S^T, dK, dV)
+  const int cq = 2 * (lane & 3);
+  bool key_ok[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int kidx = k0 + kr + 8 * r;
+    key_ok[r] = kidx < p.Skv && (!p.kmask || p.kmask[(size_t)b * p.Skv + kidx]);
+  }
+  float dv[HDP / 2], dk[HDP / 2];
+#pragma unroll
+  for (int i = 0; i < HDP / 2; ++i) dv[i] = dk[i] = 0.f;
+  mbar_wait(kv_full, 0);
+  for (int it = 0; it < n_iter; ++it) {
+    const int st = it & 1;
+    const int h = g * G + it / n_i;
+    const int qi0 = (i_begin + it % n_i) * 64;
+    const uint32_t qb = sQ + st * Cfg::QTILE, dob = sdO + st * Cfg::QTILE;
+    mbar_wait(qd_full(st), (it >> 1) & 1);
+    float sT[32], dpT[32];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < HDP / 16; ++kk) {
+      const uint32_t koff = (kk >> 2) * 16384 + (kk & 3) * 32, qoff = (kk >> 2) * 8192 + (kk & 3) * 32;
+      WgmmaSS<64, 0, 0>::mma(sT, make_smem_desc_sw128(sK + wg * 8192 + koff, 0, 1024),
+                             make_smem_desc_sw128(qb + qoff, 0, 1024), kk ? 1u : 0u);
+    }
+#pragma unroll
+    for (int kk = 0; kk < HDP / 16; ++kk) {
+      const uint32_t koff = (kk >> 2) * 16384 + (kk & 3) * 32, qoff = (kk >> 2) * 8192 + (kk & 3) * 32;
+      WgmmaSS<64, 0, 0>::mma(dpT, make_smem_desc_sw128(sV + wg * 8192 + koff, 0, 1024),
+                             make_smem_desc_sw128(dob + qoff, 0, 1024), kk ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(sT);
+    reg_fence(dpT);
+    // P^T = exp2(S^T * scale - lse) on visible (key, query) pairs, dS^T = P^T * (dP^T - delta): bf16 A fragments of
+    // dV += P^T dO and dK += dS^T Q
+    const float* lse = p.lse + ((long long)b * p.nh + h) * p.Sq;
+    const float* dlt = p.delta + ((long long)b * p.nh + h) * p.Sq;
+    uint32_t pa[4][4], da[4][4];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      float pv[4], dsv[4];
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const int qi = qi0 + 8 * jj + cq + c;
+        const bool q_ok = qi < p.Sq;
+        const float L = q_ok ? __ldg(lse + qi) : 0.f, D = q_ok ? __ldg(dlt + qi) : 0.f;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int e = 2 * r + c;
+          const bool vis = q_ok && key_ok[r] && (!p.causal || k0 + kr + 8 * r <= qi + coff);
+          const float pe = vis ? fast_exp2(fmaf(sT[4 * jj + e], p.scale_log2, -L)) : 0.f;
+          pv[e] = pe;
+          dsv[e] = pe * (dpT[4 * jj + e] - D);
+        }
+      }
+      pa[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(pv[0], pv[1]);
+      pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(pv[2], pv[3]);
+      da[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(dsv[0], dsv[1]);
+      da[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(dsv[2], dsv[3]);
+    }
+    reg_fence(dv);
+    reg_fence(dk);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {  // K = 64 queries
+      WgmmaRS<HDP, 1>::mma(dv, pa[kk], make_smem_desc_sw128(dob + kk * 2048, 8192, 1024), 1u);
+      WgmmaRS<HDP, 1>::mma(dk, da[kk], make_smem_desc_sw128(qb + kk * 2048, 8192, 1024), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(dv);
+    reg_fence(dk);
+    __syncthreads();  // this iteration's Q / dO stage is no longer read by either warpgroup
+    if (threadIdx.x == 0 && it + 2 < n_iter) load_qd(it + 2);
+  }
+  // ---- epilogue: dK (x softmax scale), dV -> bf16 (zeros for keys no query sees)
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int kidx = k0 + kr + 8 * r;
+    if (kidx >= p.Skv) continue;
+    bf16* dkp = p.dk + (long long)b * p.dk_bs + (long long)kidx * p.dk_ss + (long long)g * p.hd;
+    bf16* dvp = p.dv + (long long)b * p.dv_bs + (long long)kidx * p.dv_ss + (long long)g * p.hd;
+#pragma unroll
+    for (int jj = 0; jj < HDP / 8; ++jj) {
+      const int d = 8 * jj + cq;
+      *reinterpret_cast<__nv_bfloat162*>(dkp + d) =
+          __floats2bfloat162_rn(dk[4 * jj + 2 * r] * p.scale, dk[4 * jj + 2 * r + 1] * p.scale);
+      *reinterpret_cast<__nv_bfloat162*>(dvp + d) = __floats2bfloat162_rn(dv[4 * jj + 2 * r], dv[4 * jj + 2 * r + 1]);
+    }
+  }
+}
+
+template <int HDP>
+struct DqCfg {
+  static constexpr int ATOMS = HDP / 64;
+  static constexpr int QTILE = ATOMS * 16384;  // [128 queries x hd]
+  static constexpr int KTILE = ATOMS * 8192;   // [64 keys x hd]
+  static constexpr int STAGES = 2;
+  static constexpr int SMEM = 2 * QTILE + 2 * STAGES * KTILE + 1024 + 256;
+};
+
+template <int HDP>
+__global__ void __launch_bounds__(288, 1)
+attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                   const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, AttnBwdParams p) {
+  using Cfg = DqCfg<HDP>;
+  constexpr int STAGES = Cfg::STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t sQ = base;
+  const uint32_t sdO = sQ + Cfg::QTILE;
+  const uint32_t sK = sdO + Cfg::QTILE;
+  const uint32_t sV = sK + STAGES * Cfg::KTILE;
+  const uint32_t bars = sV + STAGES * Cfg::KTILE;
+  const uint32_t q_full = bars;
+  auto kv_full = [&](int s) { return bars + 8u * (1 + s); };
+  auto kv_empty = [&](int s) { return bars + 8u * (1 + STAGES + s); };
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q_tiles = (p.Sq + 127) / 128;
+  const int qt = q_tiles - 1 - (int)blockIdx.x;  // heavy (late) causal tiles first
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int hk = h / (p.nh / p.nkv);
+  const int q0 = qt * 128;
+  const int coff = p.Skv - p.Sq;
+  const int kv_tiles_all = (p.Skv + 63) / 64;
+  int n_tiles = kv_tiles_all;
+  if (p.causal) n_tiles = max(1, min(kv_tiles_all, (q0 + 127 + coff) / 64 + 1));
+
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+    tma_prefetch_desc(&tmdO);
+    mbar_init(q_full, 1);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(kv_full(s), 1);
+      mbar_init(kv_empty(s), 2);  // one arrive per consumer warpgroup
+    }
     mbar_fence_init();
   }
-  if (warp == 5) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem) : "r"(tmem_slot));
-  const uint32_t tA = tmem;         // S^T fp32 [128 x 128]  -> P^T bf16 packed in the first 64 columns
-  const uint32_t tB = tmem + 128;   // dP^T fp32 [128 x 128] -> dQ partial [128 q x HDP]
-  const uint32_t tdV = tmem + 256;  // [128 kv x HDP]
-  const uint32_t tdK = tmem + 384;  // [128 kv x HDP]
 
-  if (warp == 4) {
+  if (warp == 8) {
+    // ================================ TMA producer ================================
     if (lane == 0) {
-      mbar_arrive_expect_tx(kv_full, 2 * Cfg::TILE);
+      mbar_arrive_expect_tx(q_full, 2 * Cfg::QTILE);
 #pragma unroll
       for (int a = 0; a < Cfg::ATOMS; ++a) {
-        tma_load_4d(sK + a * 16384, &tmK, kv_full, a * 64, g, k0, b);
-        tma_load_4d(sV + a * 16384, &tmV, kv_full, a * 64, g, k0, b);
+        tma_load_4d(sQ + a * 16384, &tmQ, q_full, a * 64, h, q0, b);
+        tma_load_4d(sdO + a * 16384, &tmdO, q_full, a * 64, h, q0, b);
       }
-      auto load_qd = [&](int it) {
-        const int st = it & 1;
-        const int h = g * G + it / n_i;
-        const int qi0 = (i_begin + it % n_i) * 128;
-        mbar_arrive_expect_tx(qd_full(st), 2 * Cfg::TILE);
-#pragma unroll
-        for (int a = 0; a < Cfg::ATOMS; ++a) {
-          tma_load_4d(sQ + st * Cfg::TILE + a * 16384, &tmQ, qd_full(st), a * 64, h, qi0, b);
-          tma_load_4d(sdO + st * Cfg::TILE + a * 16384, &tmdO, qd_full(st), a * 64, h, qi0, b);
-        }
-      };
-      if (n_iter > 0) load_qd(0);
-      if (n_iter > 1) load_qd(1);
-      for (int it = 0; it < n_iter; ++it) {
-        // The compute warps stage the fp32 dQ partial of iteration `it` in the Q / dO stage that iteration just retired
-        // (its MMAs completed before dq_full).  This thread reduce-adds it into global memory with TMA — per-thread
-        // `red.global` on 32 different rows per instruction cost 32 % of the kernel — waits until the engine has READ the
-        // tile, and only then refills the stage with the operands of iteration it + 2 (still a full iteration ahead).
-        const int st = it & 1;
-        const int h = g * G + it / n_i;
-        const int qi0 = (i_begin + it % n_i) * 128;
-        mbar_wait(dq_staged, it & 1);
-#pragma unroll
-        for (int c = 0; c < Cfg::OCH; ++c) {
-          const uint32_t src = (c * 16384 < Cfg::TILE) ? sQ + st * Cfg::TILE + c * 16384
-                                                       : sdO + st * Cfg::TILE + (c * 16384 - Cfg::TILE);
-          tma_reduce_add_4d(&tmdQ, src, c * 32, h, qi0, b);
-        }
-        bulk_commit_group();
-        bulk_wait_group_read0();
-        if (it + 2 < n_iter) load_qd(it + 2);
-      }
-      bulk_wait_group0();
-    }
-  } else if (warp == 5) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_dv = make_idesc_bf16(128, HDP, 0, 1);   // A: P^T from TMEM, B: dO (MN-major)
-      constexpr uint32_t idesc_dk = make_idesc_bf16(128, HDP, 0, 1);   // A: dS^T smem K-major, B: Q (MN-major)
-      constexpr uint32_t idesc_dq = make_idesc_bf16(128, HDP, 1, 1);   // A: dS (MN-major view), B: K (MN-major)
-      mbar_wait(kv_full, 0);
       int st = 0;
       uint32_t ph = 0;
-      for (int it = 0; it < n_iter; ++it) {
-        mbar_wait(qd_full(st), ph);
-        if (it > 0) mbar_wait(dq_done, (it - 1) & 1);  // region B (dQ partial of it-1) has been read out
-        tc_fence_after();
-        const uint32_t qb = sQ + st * Cfg::TILE, dob = sdO + st * Cfg::TILE;
+      for (int j = 0; j < n_tiles; ++j) {
+        mbar_wait(kv_empty(st), ph ^ 1u);
+        mbar_arrive_expect_tx(kv_full(st), 2 * Cfg::KTILE);
 #pragma unroll
-        for (int kk = 0; kk < HDP / 16; ++kk) {
-          const uint32_t off = (kk >> 2) * 16384 + (kk & 3) * 32;
-          umma_ss(tA, make_smem_desc_sw128(sK + off, 0, 1024), make_smem_desc_sw128(qb + off, 0, 1024), idesc_s,
-                  kk ? 1u : 0u);
+        for (int a = 0; a < Cfg::ATOMS; ++a) {
+          tma_load_4d(sK + st * Cfg::KTILE + a * 8192, &tmK, kv_full(st), a * 64, hk, j * 64, b);
+          tma_load_4d(sV + st * Cfg::KTILE + a * 8192, &tmV, kv_full(st), a * 64, hk, j * 64, b);
         }
-#pragma unroll
-        for (int kk = 0; kk < HDP / 16; ++kk) {
-          const uint32_t off = (kk >> 2) * 16384 + (kk & 3) * 32;
-          umma_ss(tB, make_smem_desc_sw128(sV + off, 0, 1024), make_smem_desc_sw128(dob + off, 0, 1024), idesc_s,
-                  kk ? 1u : 0u);
-        }
-        umma_commit(sdp_full);
-        mbar_wait(pds_full, it & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {  // dV += P^T dO   (K = 128 queries)
-          umma_ts(tdV, tA + kk * 8, make_smem_desc_sw128(dob + kk * 2048, 16384, 1024), idesc_dv,
-                  (it | kk) ? 1u : 0u);
-        }
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {  // dK += dS^T Q
-          const uint32_t aoff = (kk >> 2) * 16384 + (kk & 3) * 32;
-          umma_ss(tdK, make_smem_desc_sw128(sdS + aoff, 0, 1024), make_smem_desc_sw128(qb + kk * 2048, 16384, 1024),
-                  idesc_dk, (it | kk) ? 1u : 0u);
-        }
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {  // dQ_i = dS K   (K = 128 keys)
-          umma_ss(tB, make_smem_desc_sw128(sdS + kk * 2048, 16384, 1024),
-                  make_smem_desc_sw128(sK + kk * 2048, 16384, 1024), idesc_dq, kk ? 1u : 0u);
-        }
-        umma_commit(dq_full);  // (the Q / dO stage is handed back through dq_staged: see the producer)
-        if (++st == 2) { st = 0; ph ^= 1u; }
+        if (++st == STAGES) { st = 0; ph ^= 1u; }
       }
     }
-  } else {
-    // 8 compute warps (0-3 and 6-9): two warps per TMEM lane quarter, each owning half of the columns of every
-    // row — the per-element work has no row reductions, so the split needs no exchange and halves the serial thread phase
-    const int row = (warp & 3) * 32 + lane;  // key row of this CTA's tile (phase 1) / query row of the tile (phase 2)
-    const int ch = warp >= 6 ? 1 : 0;        // column half
-    const int kidx = k0 + row;
-    const uint32_t lane_off = static_cast<uint32_t>((warp & 3) * 32) << 16;
-    const bool key_ok = kidx < p.Skv && (!p.kmask || p.kmask[(size_t)b * p.Skv + kidx]);
-    for (int it = 0; it < n_iter; ++it) {
-      const int h = g * G + it / n_i;
-      const int qi0 = (i_begin + it % n_i) * 128;
-      // stage lse / delta of the 128 queries of this tile (previous readers are past pds arrive of it-1)
-      {
-        const int qi = qi0 + row;
-        const long long so = ((long long)b * p.nh + h) * p.Sq + qi;
-        stat[row] = qi < p.Sq ? p.lse[so] : INFINITY;
-        stat[128 + row] = qi < p.Sq ? p.delta[so] : 0.f;
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      mbar_wait(sdp_full, it & 1);
-      tc_fence_after();
-      // queries visible to this key: qi + coff >= kidx, qi < Sq
-      int qmin = 0;
-      if (p.causal) qmin = kidx - coff - qi0;
-      const int qmax = p.Sq - qi0;
-      // P^T is written in place over S^T (columns [0, 64) of region A), i.e. over columns the OTHER half's warp still has
-      // to read: pull both S^T chunks of this warp into registers and meet at a barrier before anyone stores P^T
-      uint32_t rs2[64];
-      tmem_ld32(tA + lane_off + (2 * ch) * 32, rs2);
-      tmem_ld32(tA + lane_off + (2 * ch + 1) * 32, rs2 + 32);
-      tmem_ld_wait();
-      asm volatile("bar.sync 2, 256;" ::: "memory");
-#pragma unroll
-      for (int cc = 0; cc < 2; ++cc) {
-        const int c = 2 * ch + cc;
-        const uint32_t* rs = rs2 + cc * 32;
-        uint32_t rd[32];
-        tmem_ld32(tB + lane_off + c * 32, rd);
-        tmem_ld_wait();
-        // branch-free visibility mask for the 32 queries of this chunk
-        const int lo = max(qmin - c * 32, 0), hi = min(qmax - c * 32, 32);
-        uint32_t bits = 0u;
-        if (key_ok && hi > lo) bits = (hi >= 32 ? 0xffffffffu : ((1u << hi) - 1u)) & ~((1u << lo) - 1u);
-        float pv[32], ds[32];
-#pragma unroll
-        for (int e = 0; e < 32; ++e) {
-          const int qc = c * 32 + e;
-          float pe = fast_exp2(fmaf(__uint_as_float(rs[e]), p.scale_log2, -stat[qc]));
-          pe = ((bits >> e) & 1u) ? pe : 0.f;
-          pv[e] = pe;
-          ds[e] = pe * (__uint_as_float(rd[e]) - stat[128 + qc]);
-        }
-        // P^T -> TMEM (bf16 pairs, 16 columns per 32 queries), in place over the S^T columns already consumed
-        uint32_t pk[32];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          __nv_bfloat162 t = __floats2bfloat162_rn(pv[2 * e], pv[2 * e + 1]);
-          pk[e] = *reinterpret_cast<uint32_t*>(&t);
-        }
-        asm volatile(
-            "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-            "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-            :
-            : "r"(tA + lane_off + c * 16), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]), "r"(pk[3]), "r"(pk[4]), "r"(pk[5]),
-              "r"(pk[6]), "r"(pk[7]), "r"(pk[8]), "r"(pk[9]), "r"(pk[10]), "r"(pk[11]), "r"(pk[12]), "r"(pk[13]),
-              "r"(pk[14]), "r"(pk[15])
-            : "memory");
-        // dS^T -> smem, K-major over the 128 queries (row = key)
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const int gq = c * 4 + u;
-          const uint32_t addr = sdS + (gq >> 3) * 16384 + row * 128 + (((gq & 7) ^ (row & 7)) << 4);
-          const uint4 val = pack8(ds + u * 8);
-          asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(val.x), "r"(val.y), "r"(val.z),
-                       "r"(val.w) : "memory");
-        }
-      }
-      tmem_st_wait();
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(pds_full);
-      // ---- dQ partial: thread == query row of tile i
-      mbar_wait(dq_full, it & 1);
-      tc_fence_after();
-      {
-        // dQ partial: TMEM -> registers -> fp32 tile in this iteration's retired Q / dO stage (128B-swizzled boxes of
-        // [128 rows][32 floats], matching the reduce tensor map); the producer thread issues the TMA reduce-add
-        constexpr int HC = Cfg::OCH / 2;  // 32-column chunks of the dQ row owned by this warp
-        uint32_t r[HC * 32];
-#pragma unroll
-        for (int c = 0; c < HC; ++c) tmem_ld32(tB + lane_off + (ch * HC + c) * 32, r + c * 32);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(dq_done);  // region B is free: the next iteration's S^T / dP^T MMAs overlap with the readout below
-        const int st = it & 1;
-#pragma unroll
-        for (int rd = 0; rd < HC; ++rd) {
-          const int c = ch * HC + rd;
-          const uint32_t box = (c * 16384 < Cfg::TILE) ? sQ + st * Cfg::TILE + c * 16384
-                                                       : sdO + st * Cfg::TILE + (c * 16384 - Cfg::TILE);
-          const uint32_t dst = box + row * 128;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(dst + ((j ^ (row & 7)) << 4)),
-                         "r"(r[rd * 32 + j * 4]), "r"(r[rd * 32 + j * 4 + 1]), "r"(r[rd * 32 + j * 4 + 2]),
-                         "r"(r[rd * 32 + j * 4 + 3])
-                         : "memory");
-          }
-        }
-        fence_proxy_async_smem();
-        mbar_arrive(dq_staged);
-      }
-    }
-    // ---- epilogue: dK (x softmax scale), dV -> bf16
-    if (n_iter > 0) {
-      // dq_full of the last iteration also covers the dV / dK MMAs issued before it
-      bf16* dkp = p.dk + (long long)b * p.dk_bs + (long long)kidx * p.dk_ss + (long long)g * p.hd;
-      bf16* dvp = p.dv + (long long)b * p.dv_bs + (long long)kidx * p.dv_ss + (long long)g * p.hd;
-#pragma unroll 1
-      for (int c = ch * (Cfg::OCH / 2); c < (ch + 1) * (Cfg::OCH / 2); ++c) {
-        uint32_t r1[32], r2[32];
-        tmem_ld32(tdK + lane_off + c * 32, r1);
-        tmem_ld32(tdV + lane_off + c * 32, r2);
-        tmem_ld_wait();
-        if (kidx < p.Skv) {
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const int d0 = c * 32 + u * 8;
-            if (d0 < p.hd) {
-              float f1[8], f2[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                f1[e] = __uint_as_float(r1[u * 8 + e]) * p.scale;
-                f2[e] = __uint_as_float(r2[u * 8 + e]);
-              }
-              *reinterpret_cast<uint4*>(dkp + d0) = pack8(f1);
-              *reinterpret_cast<uint4*>(dvp + d0) = pack8(f2);
-            }
-          }
-        }
-      }
-    } else if (kidx < p.Skv) {
-      bf16* dkp = p.dk + (long long)b * p.dk_bs + (long long)kidx * p.dk_ss + (long long)g * p.hd;
-      bf16* dvp = p.dv + (long long)b * p.dv_bs + (long long)kidx * p.dv_ss + (long long)g * p.hd;
-      const uint4 z = make_uint4(0, 0, 0, 0);
-      for (int d0 = ch * (p.hd / 2); d0 < (ch + 1) * (p.hd / 2); d0 += 8) {
-        *reinterpret_cast<uint4*>(dkp + d0) = z;
-        *reinterpret_cast<uint4*>(dvp + d0) = z;
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 5) tmem_dealloc(tmem, 512);
+
+  // ================================ consumer warpgroups ================================
+  const int wg = warp >> 2;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's query rows: rloc and rloc + 8
+  const int cq = 2 * (lane & 3);
+  const uint8_t* km = p.kmask ? p.kmask + (size_t)b * p.Skv : nullptr;
+  const float* lse = p.lse + ((long long)b * p.nh + h) * p.Sq;
+  const float* dlt = p.delta + ((long long)b * p.nh + h) * p.Sq;
+  int qi[2];
+  float L[2], D[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    qi[r] = q0 + rloc + 8 * r;
+    L[r] = qi[r] < p.Sq ? __ldg(lse + qi[r]) : 0.f;
+    D[r] = qi[r] < p.Sq ? __ldg(dlt + qi[r]) : 0.f;
+  }
+  float dq[HDP / 2];
+#pragma unroll
+  for (int i = 0; i < HDP / 2; ++i) dq[i] = 0.f;
+  mbar_wait(q_full, 0);
+  int st = 0;
+  uint32_t ph = 0;
+  for (int j = 0; j < n_tiles; ++j) {
+    const int k0 = j * 64;
+    mbar_wait(kv_full(st), ph);
+    const uint32_t kb = sK + st * Cfg::KTILE, vb = sV + st * Cfg::KTILE;
+    float s[32], dp[32];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < HDP / 16; ++kk) {
+      const uint32_t qoff = wg * 8192 + (kk >> 2) * 16384 + (kk & 3) * 32, koff = (kk >> 2) * 8192 + (kk & 3) * 32;
+      WgmmaSS<64, 0, 0>::mma(s, make_smem_desc_sw128(sQ + qoff, 0, 1024), make_smem_desc_sw128(kb + koff, 0, 1024),
+                             kk ? 1u : 0u);
+    }
+#pragma unroll
+    for (int kk = 0; kk < HDP / 16; ++kk) {
+      const uint32_t qoff = wg * 8192 + (kk >> 2) * 16384 + (kk & 3) * 32, koff = (kk >> 2) * 8192 + (kk & 3) * 32;
+      WgmmaSS<64, 0, 0>::mma(dp, make_smem_desc_sw128(sdO + qoff, 0, 1024), make_smem_desc_sw128(vb + koff, 0, 1024),
+                             kk ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    reg_fence(dp);
+    // dS = P * (dP - delta), P = exp2(S * scale - lse) on visible (query, key) pairs: bf16 A fragments of dQ += dS K
+    uint32_t da[4][4];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      float dsv[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int r = e >> 1, key = k0 + 8 * jj + cq + (e & 1);
+        const bool vis = qi[r] < p.Sq && key < p.Skv && (!p.causal || key <= qi[r] + coff) && (!km || km[key]);
+        const float pe = vis ? fast_exp2(fmaf(s[4 * jj + e], p.scale_log2, -L[r])) : 0.f;
+        dsv[e] = pe * (dp[4 * jj + e] - D[r]);
+      }
+      da[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(dsv[0], dsv[1]);
+      da[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(dsv[2], dsv[3]);
+    }
+    reg_fence(dq);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)  // K = 64 keys; K read MN-major (hd contiguous)
+      WgmmaRS<HDP, 1>::mma(dq, da[kk], make_smem_desc_sw128(kb + kk * 2048, 8192, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(dq);
+    if (wg_leader) mbar_arrive(kv_empty(st));
+    if (++st == STAGES) { st = 0; ph ^= 1u; }
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    if (qi[r] >= p.Sq) continue;
+    float* dqp = p.dq_acc + (((long long)b * p.Sq + qi[r]) * p.nh + h) * p.hd;
+#pragma unroll
+    for (int jj = 0; jj < HDP / 8; ++jj)
+      *reinterpret_cast<float2*>(dqp + 8 * jj + cq) = make_float2(dq[4 * jj + 2 * r], dq[4 * jj + 2 * r + 1]);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -743,7 +649,7 @@ static int launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtens
     attr = true;
   }
   dim3 grid((p.Sq + 127) / 128, p.nh, p.B);
-  kern<<<grid, 192, Cfg::SMEM, st>>>(tq, tk, tv, p);
+  kern<<<grid, 288, Cfg::SMEM, st>>>(tq, tk, tv, p);
   CB_CUDA_LAUNCH_CHECK("attn_fwd");
   return CB_OK;
 }
@@ -775,7 +681,7 @@ int attn_fwd_launch(const void* q, const void* k, const void* v, void* o, float*
 
 template <int HDP>
 static int launch_bwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tdo,
-                      const CUtensorMap& tdq, const AttnBwdParams& p, cudaStream_t st) {
+                      const AttnBwdParams& p, cudaStream_t st) {
   using Cfg = BwdCfg<HDP>;
   auto kern = attn_bwd_kernel<HDP>;
   static bool attr = false;
@@ -785,8 +691,25 @@ static int launch_bwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtens
     attr = true;
   }
   dim3 grid((p.Skv + 127) / 128, p.nkv, p.B);
-  kern<<<grid, 320, Cfg::SMEM, st>>>(tq, tk, tv, tdo, tdq, p);
+  kern<<<grid, 256, Cfg::SMEM, st>>>(tq, tk, tv, tdo, p);
   CB_CUDA_LAUNCH_CHECK("attn_bwd");
+  return CB_OK;
+}
+
+template <int HDP>
+static int launch_bwd_dq(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tdo,
+                         const AttnBwdParams& p, cudaStream_t st) {
+  using Cfg = DqCfg<HDP>;
+  auto kern = attn_bwd_dq_kernel<HDP>;
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+    if (e != cudaSuccess) return set_error(CB_ERR_CUDA, "attn bwd dq smem attr: %s", cudaGetErrorString(e));
+    attr = true;
+  }
+  dim3 grid((p.Sq + 127) / 128, p.nh, p.B);
+  kern<<<grid, 288, Cfg::SMEM, st>>>(tq, tk, tv, tdo, p);
+  CB_CUDA_LAUNCH_CHECK("attn_bwd_dq");
   return CB_OK;
 }
 
@@ -808,36 +731,29 @@ int attn_bwd_launch(const void* q, const void* k, const void* v, const void* o, 
   }
   CUtensorMap tq, tk, tv, tdo;
   int rc;
-  if ((rc = make_tmap_bf16_4d(&tq, q, hd, nh, Sq, B, hd, q_ss, q_bs, 128))) return rc;
+  if ((rc = make_tmap_bf16_4d(&tq, q, hd, nh, Sq, B, hd, q_ss, q_bs, 64))) return rc;
   if ((rc = make_tmap_bf16_4d(&tk, k, hd, nkv, Skv, B, hd, k_ss, k_bs, 128))) return rc;
   if ((rc = make_tmap_bf16_4d(&tv, v, hd, nkv, Skv, B, hd, v_ss, v_bs, 128))) return rc;
-  if ((rc = make_tmap_bf16_4d(&tdo, d_o, hd, nh, Sq, B, hd, do_ss, do_bs, 128))) return rc;
+  if ((rc = make_tmap_bf16_4d(&tdo, d_o, hd, nh, Sq, B, hd, do_ss, do_bs, 64))) return rc;
   AttnBwdParams p;
   p.dq_acc = dq_acc; p.dk = (bf16*)dk; p.dv = (bf16*)dv;
   p.dk_bs = dk_bs; p.dk_ss = dk_ss; p.dv_bs = dv_bs; p.dv_ss = dv_ss;
   p.lse = lse; p.delta = delta; p.kmask = (const uint8_t*)kmask;
   p.B = B; p.nh = nh; p.nkv = nkv; p.Sq = Sq; p.Skv = Skv; p.hd = hd; p.causal = causal;
   p.scale_log2 = scale * LOG2E; p.scale = scale;
-  CUtensorMap tdq;  // fp32 dQ accumulator [B, Sq, nh, hd]: reduce-add target, box = 32 floats x 128 query rows
-  {
-    auto fn = encode_fn();
-    if (!fn) return set_error(CB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-    CB_CHECK_ARG((reinterpret_cast<uintptr_t>(dq_acc) & 15u) == 0, "attention bwd: dq_acc must be 16-byte aligned");
-    cuuint64_t dims[4] = {(cuuint64_t)hd, (cuuint64_t)nh, (cuuint64_t)Sq, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)hd * 4, (cuuint64_t)nh * hd * 4, (cuuint64_t)Sq * nh * hd * 4};
-    cuuint32_t box[4] = {32, 1, 128, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = CUDA_SUCCESS;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-      r = fn(&tdq, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, dq_acc, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_ERROR_INVALID_CONTEXT) break;
-      cudaFree(0);
-    }
-    if (r != CUDA_SUCCESS) return set_error(CB_ERR_CUDA, "cuTensorMapEncodeTiled(dq) failed (%d)", (int)r);
+  CB_CHECK_ARG((reinterpret_cast<uintptr_t>(dq_acc) & 7u) == 0, "attention bwd: dq_acc must be 8-byte aligned");
+  // the dQ kernel streams 64-key K / V tiles against 128-query Q / dO tiles
+  CUtensorMap tq128, tk64, tv64, tdo128;
+  if ((rc = make_tmap_bf16_4d(&tq128, q, hd, nh, Sq, B, hd, q_ss, q_bs, 128))) return rc;
+  if ((rc = make_tmap_bf16_4d(&tk64, k, hd, nkv, Skv, B, hd, k_ss, k_bs, 64))) return rc;
+  if ((rc = make_tmap_bf16_4d(&tv64, v, hd, nkv, Skv, B, hd, v_ss, v_bs, 64))) return rc;
+  if ((rc = make_tmap_bf16_4d(&tdo128, d_o, hd, nh, Sq, B, hd, do_ss, do_bs, 128))) return rc;
+  if (hd == 64) {
+    if ((rc = launch_bwd<64>(tq, tk, tv, tdo, p, st))) return rc;
+    return launch_bwd_dq<64>(tq128, tk64, tv64, tdo128, p, st);
   }
-  if (hd == 64) return launch_bwd<64>(tq, tk, tv, tdo, tdq, p, st);
-  return launch_bwd<128>(tq, tk, tv, tdo, tdq, p, st);
+  if ((rc = launch_bwd<128>(tq, tk, tv, tdo, p, st))) return rc;
+  return launch_bwd_dq<128>(tq128, tk64, tv64, tdo128, p, st);
 }
 
 }  // namespace cb

@@ -1,16 +1,16 @@
-// cambrian_b200 — shared device helpers for sm_100a (B200).
+// cambrian_b200 — shared device helpers for sm_90a (H100).
 //
-// Thin inline-PTX wrappers for the Blackwell machinery every dense kernel in this
-// library uses: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit /
-// ld / fences) and the UMMA shared-memory + instruction descriptors.  Nothing here is
+// Thin inline-PTX wrappers for the Hopper machinery every dense kernel in this library
+// uses: mbarrier, TMA (cp.async.bulk.tensor), wgmma (fences, groups, shared-memory
+// descriptors; the MMA instructions themselves are in wgmma.cuh).  Nothing here is
 // derived from the reference (which ships no native code, SURVEY.md §2a); bit layouts
-// follow the PTX ISA as restated in the vendored CUTLASS headers
-// (cute/arch/mma_sm100_desc.hpp: SmemDescriptor, InstrDescriptor).
+// follow the PTX ISA (wgmma matrix descriptors, canonical SWIZZLE_128B layouts).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <cuda.h>
 #include <stdint.h>
+#include "wgmma.cuh"
 
 namespace cb {
 
@@ -80,7 +80,7 @@ __device__ __forceinline__ float erf_fast(float x) {
   return copysignf(r, x);
 }
 // x * Phi(x) with the same A&S erf, constants folded for z = x / sqrt(2): 14 instructions (2 MUFU) per element —
-// GELU epilogues are ALU-bound (profiles/r01_gemm_epilogue_microbench.log), so every instruction shows
+// GELU epilogues are ALU-bound, so every instruction shows
 __device__ __forceinline__ float gelu_erf(float x) {
   const float ax = fabsf(x);
   const float t = fast_rcp(fmaf(0.3275911f * 0.70710678118654752440f, ax, 1.0f));
@@ -173,7 +173,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         : "memory");
   } while (!done);
 }
-// generic-proxy writes to smem -> visible to the async proxy (TMA store / UMMA reads)
+// generic-proxy writes to smem -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -184,26 +184,6 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
 }
-// TMA store (smem tile -> global), bulk-group completion; rows / columns outside the tensor are clipped by the engine
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-               :
-               : "l"(m), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_wait_group_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
-// TMA reduce-add (smem tile -> global, element-wise += in L2), bulk-group completion
-__device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1, int c2,
-                                                  int c3) {
-  asm volatile(
-      "cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-      :
-      : "l"(m), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap* m, uint32_t bar,
                                             int c0, int c1, int c2) {
   asm volatile(
@@ -224,205 +204,32 @@ __device__ __forceinline__ void tma_load_4d(uint32_t smem_dst, const CUtensorMap
 }
 
 // ----------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (sm_90a warpgroup MMA): ordering fences and group completion
 // ----------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_slot),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// register accumulators / A fragments written by ordinary instructions -> visible to the next wgmma.mma_async
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]   (kind::f16: bf16/fp16 inputs, fp32 accumulate)
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n"
-      :
-      : "r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// all previously issued tcgen05.mma of this thread complete -> arrive(1) on mbarrier
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-// warp-collective: lane i of the warp reads TMEM lane (base_lane + i), 32 consecutive columns
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-      :
-      : "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]),
-        "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]),
-        "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]),
-        "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]),
-        "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // ----------------------------------------------------------------------------------
-// CTA-pair (cta_group::2) variants: two CTAs of a (2,1,1) cluster cooperate on one 256-row MMA tile.
-// PTX forms as in the vendored CUTLASS headers (cute/arch/copy_sm100_tma.hpp SM100_TMA_2SM_LOAD_3D,
-// cutlass/arch/barrier.h umma_arrive_multicast_2x1SM, cute/arch/tmem_allocator_sm100.hpp Allocator2Sm).
-// ----------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  // non-.aligned forms: the single-lane producer / MMA roles leave their warps diverged when the others get here
-  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_slot), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// issued by the leader CTA only: D (256 x N, rows split over the two CTAs' TMEM) (+)= A (each CTA's 128 rows) * B (each
-// CTA holds N/2 rows); descriptors are CTA-local smem offsets applied in both CTAs
-__device__ __forceinline__ void umma_ss_2cta(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive(1) on the barrier at the same smem offset in every CTA of `mask` once all prior MMAs of this thread retire
-__device__ __forceinline__ void umma_commit_2cta_mc(uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-      "h"(mask)
-      : "memory");
-}
-// TMA load into THIS CTA's smem whose transaction bytes are credited to the LEADER CTA's mbarrier (peer bit cleared)
-__device__ __forceinline__ void tma_load_3d_2cta(uint32_t smem_dst, const CUtensorMap* m, uint32_t bar, int c0, int c1,
-                                                 int c2) {
-  const uint32_t leader_bar = bar & 0xFEFFFFFFu;
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4, %5}], [%2];"
-      :
-      : "r"(smem_dst), "l"(m), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
-  asm volatile(
-      "{\n"
-      ".reg .b32 rem;\n"
-      "mapa.shared::cluster.u32 rem, %0, %1;\n"
-      "mbarrier.arrive.shared::cluster.b64 _, [rem];\n"
-      "}\n"
-      :
-      : "r"(bar), "r"(cta)
-      : "memory");
-}
-
-// ----------------------------------------------------------------------------------
-// Cluster Launch Control (sm_100): a running CTA asks the hardware work distributor to CANCEL a not-yet-launched
-// CTA / cluster of its own grid and takes over that block index.  A grid of one CTA per output tile then behaves like a
-// persistent kernel with a hardware tile queue: SMs that are busy with somebody else's kernel (an NCCL collective, an
-// optimizer grid) simply never receive a CTA and their share of the tiles is picked up by the SMs that are free.
-// PTX forms as in the vendored CUTLASS (cutlass/gemm/kernel/sm100_tile_scheduler.hpp: issue_clc_query /
-// work_tile_info_from_clc_response).
-// ----------------------------------------------------------------------------------
-// asynchronous: writes a 16-byte response to `resp` (this CTA) and completes 16 tx bytes on `bar`
-__device__ __forceinline__ void clc_try_cancel(uint32_t resp, uint32_t bar) {
-  asm volatile("clusterlaunchcontrol.try_cancel.async.shared::cta.mbarrier::complete_tx::bytes.b128 [%0], [%1];" ::"r"(resp),
-               "r"(bar)
-               : "memory");
-}
-// cluster variant: response + completion are multicast to the same offsets in EVERY CTA of the cluster
-__device__ __forceinline__ void clc_try_cancel_multicast(uint32_t resp, uint32_t bar) {
-  asm volatile(
-      "clusterlaunchcontrol.try_cancel.async.shared::cta.mbarrier::complete_tx::bytes.multicast::cluster::all.b128 [%0], [%1];" ::
-          "r"(resp),
-      "r"(bar)
-      : "memory");
-}
-// decode a response: blockIdx.x of the cancelled CTA (first CTA of the cancelled cluster), or -1 if nothing was left
-__device__ __forceinline__ int clc_decode(uint32_t resp) {
-  uint32_t x = 0, y = 0, z = 0, ok = 0;
-  asm volatile(
-      "{\n"
-      ".reg .pred p1;\n"
-      ".reg .b128 clc_result;\n"
-      "ld.shared.b128 clc_result, [%4];\n"
-      "clusterlaunchcontrol.query_cancel.is_canceled.pred.b128 p1, clc_result;\n"
-      "selp.u32 %3, 1, 0, p1;\n"
-      "@p1 clusterlaunchcontrol.query_cancel.get_first_ctaid.v4.b32.b128 {%0, %1, %2, _}, clc_result;\n"
-      "}\n"
-      : "=r"(x), "=r"(y), "=r"(z), "=r"(ok)
-      : "r"(resp)
-      : "memory");
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic read ordered before the next async write
-  return ok ? static_cast<int>(x) : -1;
-}
-
-// ----------------------------------------------------------------------------------
-// UMMA descriptors (SWIZZLE_128B canonical layouts, bf16)
+// wgmma shared-memory descriptors (SWIZZLE_128B canonical layouts, bf16)
 //
 // K-major tile (rows = M or N, 64 bf16 = 128 B of K per row, rows packed at 128 B):
 //     8-row groups are 1024 B apart -> SBO = 1024, LBO unused.
 //     advancing K by 16 elements inside the 128-B swizzle atom = +32 B on the start address.
-// MN-major tile (rows = K, 64 bf16 = 128 B of M/N per row; one TMA box = 64(MN) x BLOCK_K):
+// MN-major tile (rows = K, 64 bf16 = 128 B of M/N per row; one TMA box = 64(MN) x rows):
 //     8-row K groups are 1024 B apart -> SBO = 1024; the next 64-wide MN atom is a whole
-//     box away -> LBO = BLOCK_K * 128.  advancing K by 16 rows = +2048 B.
+//     box away -> LBO = box bytes.  advancing K by 16 rows = +2048 B.
+// Tiles start on 1024-byte boundaries, so the swizzle phase is a function of the address (base offset 0).
 // ----------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes,
                                                          uint32_t sbo_bytes) {
@@ -430,20 +237,14 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);              // [0,14)  start address
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;     // [16,30) leading byte offset
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;     // [32,46) stride byte offset
-  d |= static_cast<uint64_t>(1) << 46;                              // [46,48) version = 1 (sm100)
-  d |= static_cast<uint64_t>(2) << 61;                              // [61,64) SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                              // [62,64) layout: SWIZZLE_128B
   return d;
 }
-// kind::f16 instruction descriptor: bf16 x bf16 -> fp32
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t m, uint32_t n, uint32_t a_mn_major,
-                                                       uint32_t b_mn_major) {
-  return (1u << 4)                  // c_format  = F32
-         | (1u << 7)                // a_format  = BF16
-         | (1u << 10)               // b_format  = BF16
-         | (a_mn_major << 15)       // a_major   (0 = K-major, 1 = MN-major)
-         | (b_mn_major << 16)       // b_major
-         | ((n >> 3) << 17)         // n_dim
-         | ((m >> 4) << 24);        // m_dim
+
+// two fp32 -> one bf16x2 register (low half = first element): the A-fragment format of wgmma with A in registers
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+  __nv_bfloat162 t = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&t);
 }
 
 }  // namespace cb

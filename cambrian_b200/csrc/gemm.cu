@@ -1,4 +1,4 @@
-// cambrian_b200 — persistent warp-specialised tcgen05 GEMM for sm_100a.
+// cambrian_b200 — warp-specialised wgmma GEMM for sm_90a (H100).
 //
 //   C[b] (M x N, row-major)  (+)=  epilogue( alpha * A[b] (M x K) * B[b] (K x N) )
 //
@@ -8,24 +8,25 @@
 // GEMMs (dX = dY*W, dW = dY^T*X), which is why both operands can be K-major or MN-major:
 //     a_mn = 0 : A stored [M, K] (K contiguous)       a_mn = 1 : A stored [K, M] (M contiguous)
 //     b_mn = 0 : B stored [N, K] (nn.Linear weight)   b_mn = 1 : B stored [K, N] (N contiguous)
+// wgmma reads either major straight from shared memory (the transpose bits of the instruction), so no layout
+// needs a transposed copy.
 //
-// Structure (one CTA per SM, 320 threads):
-//     warp 0      TMA producer   : cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx
-//     warp 1      MMA issuer     : one lane issues tcgen05.mma 128 x BN x 16, accumulators in TMEM
-//     warps 2..9  epilogue       : tcgen05.ld TMEM -> regs -> bias / act / scale / residual -> HBM
-//                                  (two warps per TMEM lane quarter, each owning half of the tile's columns, so an
-//                                   activation-heavy epilogue such as GELU keeps up with short-K mainloops)
-// The TMEM accumulator is double-buffered so the epilogue of tile i overlaps the MMAs of tile i+1.
+// Structure (one CTA per 128 x BN output tile, 288 threads):
+//     warp 8      TMA producer   : cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx
+//     warps 0..7  two consumer warpgroups, 64 rows each: wgmma.mma_async 64 x BN x 16 with fp32 accumulators in
+//                 registers, one k-block group kept in flight, then bias / act / scale / residual -> HBM
+// BN = 64 / 128 / 256 is chosen per problem so that small GEMMs still put a CTA on most of the 132 SMs.
 #include "common.cuh"
 #include <cstring>
 #include <cudaTypedefs.h>
 #include <mutex>
-#include <cstdlib>
 
 namespace cb {
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 B = one SWIZZLE_128B atom
+constexpr int GEMM_THREADS = 288;
+constexpr int GROUP_M = 16;  // tile rasterisation: super-rows of 16 m-blocks (2048 rows) keep their A panel L2-resident
 
 struct GemmEpilogue {
   void* C;
@@ -35,17 +36,13 @@ struct GemmEpilogue {
   const bf16* residual;  // [M, N] or null
   long long ldr, bsr;
   float alpha;
-  int act;         // 0 none, 1 gelu(erf), 2 gelu(tanh), 3 quick_gelu, 4 silu
   int out_fp32;    // C dtype: 0 bf16, 1 fp32
   int accumulate;  // C += result
-  int vec_ok;      // 16-byte vector stores are legal
-  int group_m;     // tile rasterisation: 0 = m fastest over all m-blocks; g > 0 = super-rows of g m-blocks (L2 reuse of A)
-  int tma_store;   // bf16 output without accumulate: tiles leave through smem staging + TMA stores (tmC / tmAux)
-  void* aux;       // ACT_SWIGLU_PAIR: second output, silu(gate) * up, [M, N / 2] bf16
+  int pair_ok;     // two adjacent columns can be loaded / stored as one 4-byte (bf16) / 8-byte (fp32) access
+  void* aux;       // fused SwiGLU: second output, silu(gate) * up, [M, N / 2] bf16
   long long ld_aux;
-  int dyn;         // 1: one CTA (pair) per tile in the grid, tiles handed out by Cluster Launch Control (TileRing below)
 };
-constexpr int ACT_SWIGLU_PAIR = 5;  // CTA-pair kernel only: the tile's two B halves are gate rows and the matching up rows
+constexpr int ACT_SWIGLU_PAIR = 5;  // the tile's two B halves are 64 gate rows and the matching 64 up rows
 
 template <int BN>
 struct GemmCfg {
@@ -53,12 +50,11 @@ struct GemmCfg {
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
-  static constexpr int TMEM_COLS = 2 * BN;  // 512 / 256 / 128 — powers of two
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 1024 /*barriers*/ + 32768 /*store staging*/;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
 // activation selected at COMPILE time: a per-element runtime switch (plus slow-path erff / tanhf) made the epilogue of
-// short-K GEMMs 3.4x slower than their mainloop (profiles/r01_gemm_epilogue_microbench.log)
+// short-K GEMMs several times slower than their mainloop
 template <int ACT>
 __device__ __forceinline__ float apply_act(float v) {
   if constexpr (ACT == 1) return gelu_erf(v);
@@ -68,761 +64,231 @@ __device__ __forceinline__ float apply_act(float v) {
   else return v;
 }
 
-
-// tile index -> (m block, n block).  group_m > 0 walks the output in super-rows of group_m m-blocks (all n-blocks of a
-// super-row before the next one) so that a super-row's A panel stays L2-resident while B streams through once per
-// super-row; group_m = 0 keeps one n-block column at a time (B resident, A re-read per column).
-__device__ __forceinline__ void tile_to_mn(int r, int m_blocks, int n_blocks, int group_m, int& mb, int& nb) {
-  if (group_m <= 0) {
-    mb = r % m_blocks;
-    nb = r / m_blocks;
-    return;
-  }
-  const int tpg = group_m * n_blocks;
+// tile index -> (m block, n block): super-rows of GROUP_M m-blocks (all n-blocks of a super-row before the next one), so
+// that a super-row's A panel stays L2-resident while B streams through once per super-row.
+__device__ __forceinline__ void tile_to_mn(int r, int m_blocks, int n_blocks, int& mb, int& nb) {
+  const int tpg = GROUP_M * n_blocks;
   const int g = r / tpg;
-  const int first = g * group_m;
-  const int gs = min(group_m, m_blocks - first);
+  const int first = g * GROUP_M;
+  const int gs = min(GROUP_M, m_blocks - first);
   const int w = r - g * tpg;
   mb = first + w % gs;
   nb = w / gs;
 }
 
-// ------------------------------------------------------------------------------------------
-// Dynamic tile scheduling (ep.dyn).  The grid holds ONE CTA (CTA pair) PER TILE.  A CTA that gets to run works on its own
-// block index first; its TMA-producer thread then keeps asking Cluster Launch Control to cancel a still-pending CTA of the
-// grid and processes that CTA's tile instead (common.cuh: clc_*), until nothing is pending.  Each tile id is handed to the
-// CTA's other roles (MMA issuer, 8 epilogue warps) through an 8-slot shared-memory ring guarded by full / empty mbarriers;
-// -1 ends every role's loop.  Compared with the static `tile += gridDim.x` walk of a 148-CTA persistent grid this makes
-// the GEMM indifferent to SMs it does not get: when an NCCL collective or the background optimizer holds some SMs, fewer
-// CTAs become resident and the resident ones simply take more tiles, instead of a late CTA still owning 1/148 of the
-// work (r01: that cost the full all-reduce time at every N, SCALE_r01).  The CLC query for the NEXT tile is in flight
-// while the current tile's operands stream in.
-// ------------------------------------------------------------------------------------------
-constexpr int RING = 8;
-struct TileRing {
-  uint32_t ids, full, empty, resp, clc_bar, clc_empty;
-};
-__device__ __forceinline__ TileRing make_ring(uint32_t bar_base) {
-  TileRing r;
-  r.ids = bar_base + 256u;         // int[RING]
-  r.full = bar_base + 320u;        // mbarrier[RING], 1 arrival (producer thread)
-  r.empty = bar_base + 384u;       // mbarrier[RING], 9 arrivals (MMA-warp lane + 8 epilogue warps)
-  r.resp = bar_base + 512u;        // 16-byte CLC response
-  r.clc_bar = bar_base + 528u;     // mbarrier: CLC response landed (16 tx bytes)
-  r.clc_empty = bar_base + 536u;   // pair kernel, leader's copy: the peer CTA has decoded the previous response
-  return r;
-}
-__device__ __forceinline__ void ring_init(const TileRing& r) {
-  for (int s = 0; s < RING; ++s) {
-    mbar_init(r.full + 8u * s, 1);
-    mbar_init(r.empty + 8u * s, 9);
-  }
-  mbar_init(r.clc_bar, 1);
-  mbar_init(r.clc_empty, 1);
-}
-__device__ __forceinline__ void ring_publish(const TileRing& r, int it, int tile) {
-  const int s = it & (RING - 1);
-  mbar_wait(r.empty + 8u * s, static_cast<uint32_t>(((it / RING) & 1) ^ 1));
-  asm volatile("st.shared.s32 [%0], %1;" ::"r"(r.ids + 4u * s), "r"(tile) : "memory");
-  mbar_arrive(r.full + 8u * s);  // release: the id is visible to whoever observes the phase
-}
-// one thread
-__device__ __forceinline__ int ring_fetch(const TileRing& r, int it) {
-  const int s = it & (RING - 1);
-  mbar_wait(r.full + 8u * s, static_cast<uint32_t>((it / RING) & 1));
-  int t;
-  asm volatile("ld.shared.s32 %0, [%1];" : "=r"(t) : "r"(r.ids + 4u * s) : "memory");
-  mbar_arrive(r.empty + 8u * s);
-  return t;
-}
-// whole warp (every lane needs the id); one arrival per warp
-__device__ __forceinline__ int ring_fetch_warp(const TileRing& r, int it, int lane) {
-  const int s = it & (RING - 1);
-  mbar_wait(r.full + 8u * s, static_cast<uint32_t>((it / RING) & 1));
-  int t;
-  asm volatile("ld.shared.s32 %0, [%1];" : "=r"(t) : "r"(r.ids + 4u * s) : "memory");
-  __syncwarp();
-  if (lane == 0) mbar_arrive(r.empty + 8u * s);
-  return t;
-}
-
-// Epilogue of one accumulator tile for the 32-column chunks [c_begin, c_end) owned by this warp:
-// tcgen05.ld -> alpha, bias, activation, LayerScale, residual, accumulate -> bf16 / fp32 stores.
-// Output staging for TMA stores.  Each epilogue warp owns two 2 KB buffers holding a [32 rows][32 bf16] tile in the
-// SWIZZLE_64B layout of the output tensor map (16-byte chunk j of row r lives at chunk j ^ ((r >> 1) & 3)), fills one
-// with st.shared (conflict-free per quarter-warp) and lets lane 0 issue the bulk store.  Direct st.global from the
-// tcgen05.ld register layout writes 16 bytes to each of 32 different rows per instruction; those uncoalesced stores
-// share the L1 data path with the TMA operand fills and cost the gate/up GEMM 8 % once its output grew by a third
-// (profiles/r01_gemm_store_path.log).
-struct StageRing {
-  uint32_t base;  // this warp's 4 KB
-  int k;          // tiles issued so far
-};
-__device__ __forceinline__ void stage_store_tile(StageRing& ring, int lane, const CUtensorMap* tm, int col0, int row0,
-                                                 int b, const uint4 (&v)[4]) {
-  const uint32_t buf = ring.base + (ring.k & 1) * 2048;
-  if (ring.k >= 2) {  // the store issued two tiles ago used this buffer: wait until the engine has read it
-    if (lane == 0) bulk_wait_group_read1();
-    __syncwarp();
-  }
-  const uint32_t dst = buf + lane * 64;
-  const int sw = (lane >> 1) & 3;
-#pragma unroll
-  for (int j = 0; j < 4; ++j)
-    asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(dst + ((j ^ sw) << 4)), "r"(v[j].x), "r"(v[j].y),
-                 "r"(v[j].z), "r"(v[j].w)
-                 : "memory");
-  fence_proxy_async_smem();
-  __syncwarp();
-  if (lane == 0) {
-    tma_store_3d(tm, buf, col0, row0, b);
-    bulk_commit_group();
-  }
-  ++ring.k;
-}
-
-#ifndef CB_EPI_INNER
-#define CB_EPI_INNER 1  // measured: 1 beats 2 and 4 (profiles/r01_gemm_epilogue_microbench.log) — code size matters more than ILP
-#endif
-
-// Rare path (N % 8 != 0 or a misaligned vector operand): element-at-a-time through a local array, deliberately NOT
-// unrolled — the unrolled scalar fallbacks used to triple the kernel's code size (210 KB of SASS, instruction-cache
-// misses on the hot path, profiles/r01_gemm_epilogue_microbench.log).
+// one output element pair (columns col, col + 1 of one row): alpha, bias, activation, LayerScale, residual, accumulate
 template <int ACT>
-__device__ __noinline__ void epilogue_chunk_scalar(const GemmEpilogue& ep, const uint32_t* rr, long long c_off,
-                                                   long long r_off, int col0, int N) {
-  const int n = min(32, N - col0);
-#pragma unroll 1
-  for (int j = 0; j < n; ++j) {
-    const int col = col0 + j;
-    float v = __uint_as_float(rr[j]) * ep.alpha;
-    if (ep.bias) v += __bfloat162float(ep.bias[col]);
-    v = apply_act<ACT>(v);
-    if (ep.colscale) v *= __bfloat162float(ep.colscale[col]);
-    if (ep.residual) v += __bfloat162float(ep.residual[r_off + col]);
+__device__ __forceinline__ void epilogue_pair(const GemmEpilogue& ep, long long c_off, long long r_off, int col, int N,
+                                              float v0, float v1) {
+  v0 *= ep.alpha;
+  v1 *= ep.alpha;
+  if (ep.pair_ok) {
+    if (col >= N) return;  // N is even here, so col + 1 < N as well
+    if (ep.bias) {
+      const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ep.bias + col));
+      v0 += t.x;
+      v1 += t.y;
+    }
+    v0 = apply_act<ACT>(v0);
+    v1 = apply_act<ACT>(v1);
+    if (ep.colscale) {
+      const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ep.colscale + col));
+      v0 *= t.x;
+      v1 *= t.y;
+    }
+    if (ep.residual) {
+      const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ep.residual + r_off + col));
+      v0 += t.x;
+      v1 += t.y;
+    }
     if (ep.out_fp32) {
-      float* cp = reinterpret_cast<float*>(ep.C) + c_off + col;
+      float2* cp = reinterpret_cast<float2*>(reinterpret_cast<float*>(ep.C) + c_off + col);
+      if (ep.accumulate) {
+        const float2 o = *cp;
+        v0 += o.x;
+        v1 += o.y;
+      }
+      *cp = make_float2(v0, v1);
+    } else {
+      __nv_bfloat162* cp = reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<bf16*>(ep.C) + c_off + col);
+      if (ep.accumulate) {
+        const float2 o = __bfloat1622float2(*cp);
+        v0 += o.x;
+        v1 += o.y;
+      }
+      *cp = __floats2bfloat162_rn(v0, v1);
+    }
+    return;
+  }
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {  // odd N or a misaligned operand: element by element
+    const int c = col + e;
+    if (c >= N) break;
+    float v = e ? v1 : v0;
+    if (ep.bias) v += __bfloat162float(ep.bias[c]);
+    v = apply_act<ACT>(v);
+    if (ep.colscale) v *= __bfloat162float(ep.colscale[c]);
+    if (ep.residual) v += __bfloat162float(ep.residual[r_off + c]);
+    if (ep.out_fp32) {
+      float* cp = reinterpret_cast<float*>(ep.C) + c_off + c;
       *cp = ep.accumulate ? *cp + v : v;
     } else {
-      bf16* cp = reinterpret_cast<bf16*>(ep.C) + c_off + col;
+      bf16* cp = reinterpret_cast<bf16*>(ep.C) + c_off + c;
       *cp = __float2bfloat16(ep.accumulate ? __bfloat162float(*cp) + v : v);
     }
   }
 }
 
-template <int BN, int ACT>
-__device__ __forceinline__ void epilogue_columns(const GemmEpilogue& ep, uint32_t taddr, int row, bool row_ok, int b,
-                                                 int n0, int N, int c_begin, StageRing& ring, const CUtensorMap* tmC,
-                                                 int row0, int lane) {
-  // One warp drains NCH 32-column chunks of its 32 accumulator rows, software-pipelined: the tcgen05.ld of chunk i+1 and
-  // the bias / column-scale / residual vectors of chunk i are in flight while chunk i's arithmetic runs — with only two
-  // epilogue warps per scheduler nothing else hides those latencies.
-  constexpr int NCH = BN / 64;
-  const long long c_off = static_cast<long long>(b) * ep.bsc + static_cast<long long>(row) * ep.ldc;
-  const long long r_off = static_cast<long long>(b) * ep.bsr + static_cast<long long>(row) * ep.ldr;
-  const bool vec = ep.vec_ok;  // N % 8 == 0 and 16-byte aligned vectors (host-checked)
-  const bool has_bias = ep.bias != nullptr, has_scale = ep.colscale != nullptr;
-  const bool has_res = ep.residual != nullptr, has_alpha = ep.alpha != 1.0f;
-  // chunks are unrolled (and pipelined) in groups of INNER; the group loop itself is not unrolled to bound code size
-  constexpr int INNER = NCH < CB_EPI_INNER ? NCH : CB_EPI_INNER;
-  uint32_t rr[2][32];
-#pragma unroll 1
-  for (int o = 0; o < NCH; o += INNER) {
-  if (n0 + (c_begin + o) * 32 >= N) break;  // warp-uniform
-  tmem_ld32(taddr + (c_begin + o) * 32, rr[0]);
-#pragma unroll
-  for (int i = 0; i < INNER; ++i) {
-    const int c = c_begin + o + i;
-    const int col0 = n0 + c * 32;
-    if (col0 >= N) break;  // warp-uniform
-    uint4 qb[4], qs[4], qr[4];
-    if (vec) {
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const int col = col0 + g * 8;
-        if (col < N) {
-          if (has_bias) qb[g] = *reinterpret_cast<const uint4*>(ep.bias + col);
-          if (has_scale) qs[g] = *reinterpret_cast<const uint4*>(ep.colscale + col);
-          if (has_res && row_ok) qr[g] = ldg_nc(ep.residual + r_off + col);
-        }
-      }
-    }
-    tmem_ld_wait();
-    if (i + 1 < INNER && col0 + 32 < N) tmem_ld32(taddr + (c + 1) * 32, rr[(i + 1) & 1]);
-    if (ep.tma_store) {
-      // whole warp participates (rows / columns past the edge are clipped by the store engine)
-      uint4 tile[4];
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const int col = col0 + g * 8;
-        float v[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(rr[i & 1][g * 8 + j]);
-        if (has_alpha) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) v[j] *= ep.alpha;
-        }
-        if (col < N) {
-          if (has_bias) {
-            float t[8];
-            unpack8(qb[g], t);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] += t[j];
-          }
-          if (ACT != 0) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = apply_act<ACT>(v[j]);
-          }
-          if (has_scale) {
-            float t[8];
-            unpack8(qs[g], t);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] *= t[j];
-          }
-          if (has_res && row_ok) {
-            float t[8];
-            unpack8(qr[g], t);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] += t[j];
-          }
-        }
-        tile[g] = pack8(v);
-      }
-      stage_store_tile(ring, lane, tmC, col0, row0, b, tile);
-      continue;
-    }
-    if (!row_ok) continue;
-    if (!vec) {
-      epilogue_chunk_scalar<ACT>(ep, rr[i & 1], c_off, r_off, col0, N);
-      continue;
-    }
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      const int col = col0 + g * 8;
-      if (col >= N) break;
-      float v[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(rr[i & 1][g * 8 + j]);
-      if (has_alpha) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] *= ep.alpha;
-      }
-      if (has_bias) {
-        float t[8];
-        unpack8(qb[g], t);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] += t[j];
-      }
-      if (ACT != 0) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = apply_act<ACT>(v[j]);
-      }
-      if (has_scale) {
-        float t[8];
-        unpack8(qs[g], t);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] *= t[j];
-      }
-      if (has_res) {
-        float t[8];
-        unpack8(qr[g], t);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] += t[j];
-      }
-      if (ep.out_fp32) {
-        float4* c4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(ep.C) + c_off + col);
-        if (ep.accumulate) {
-          const float4 o0 = c4[0], o1 = c4[1];
-          v[0] += o0.x; v[1] += o0.y; v[2] += o0.z; v[3] += o0.w;
-          v[4] += o1.x; v[5] += o1.y; v[6] += o1.z; v[7] += o1.w;
-        }
-        c4[0] = make_float4(v[0], v[1], v[2], v[3]);
-        c4[1] = make_float4(v[4], v[5], v[6], v[7]);
-      } else {
-        bf16* cp = reinterpret_cast<bf16*>(ep.C) + c_off + col;
-        if (ep.accumulate) {
-          float t[8];
-          unpack8(*reinterpret_cast<const uint4*>(cp), t);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) v[j] += t[j];
-        }
-        *reinterpret_cast<uint4*>(cp) = pack8(v);
-      }
-    }
-  }
-  }
-}
-
-// LLaMA MLP first half fused (cambrian_llama.py:142-166 -> HF LlamaMLP): B = [gate_proj; up_proj] (N = 2F rows).  The
-// CTA pair's tile takes gate rows [nb*128, +128) from CTA 0's B half and up rows [F + nb*128, +128) from CTA 1's, so
-// accumulator columns [0,128) / [128,256) hold gate / up of the SAME 128 features: the epilogue writes both
-// pre-activations (saved for backward) and silu(gate) * up without a second pass over the [M, 2F] tensor.
-__device__ __forceinline__ void epilogue_swiglu_pair(const GemmEpilogue& ep, uint32_t taddr, int row, bool row_ok, int nb,
-                                                     int N, int col_half, StageRing& ring, const CUtensorMap* tmC,
-                                                     const CUtensorMap* tmAux, int row0, int lane) {
-  const int F = N >> 1;
-  bf16* gu = reinterpret_cast<bf16*>(ep.C) + static_cast<long long>(row) * ep.ldc;
-  bf16* ao = reinterpret_cast<bf16*>(ep.aux) + static_cast<long long>(row) * ep.ld_aux;
-#pragma unroll 1
-  for (int i = 0; i < 2; ++i) {
-    const int c = col_half * 2 + i;             // 32-column chunk of the 128 features of this tile
-    const int f0 = nb * 128 + c * 32;           // feature index
-    if (f0 >= F) break;                         // warp-uniform
-    uint32_t rg[32], ru[32];
-    tmem_ld32(taddr + c * 32, rg);
-    tmem_ld32(taddr + 128 + c * 32, ru);
-    tmem_ld_wait();
-    if (ep.tma_store) {
-      uint4 tg[4], tu[4], to[4];
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        float a[8], u[8], o[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          a[j] = __bfloat162float(__float2bfloat16(__uint_as_float(rg[g * 8 + j])));
-          u[j] = __bfloat162float(__float2bfloat16(__uint_as_float(ru[g * 8 + j])));
-          o[j] = silu(a[j]) * u[j];
-        }
-        tg[g] = pack8(a);
-        tu[g] = pack8(u);
-        to[g] = pack8(o);
-      }
-      stage_store_tile(ring, lane, tmC, f0, row0, 0, tg);
-      stage_store_tile(ring, lane, tmC, F + f0, row0, 0, tu);
-      stage_store_tile(ring, lane, tmAux, f0, row0, 0, to);
-      continue;
-    }
-    if (!row_ok) continue;
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      const int f = f0 + g * 8;
-      if (f >= F) break;
-      float a[8], u[8], o[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        // round to bf16 first: the separate kernels (and the reference) apply silu to the STORED bf16 pre-activations
-        a[j] = __bfloat162float(__float2bfloat16(__uint_as_float(rg[g * 8 + j])));
-        u[j] = __bfloat162float(__float2bfloat16(__uint_as_float(ru[g * 8 + j])));
-        o[j] = silu(a[j]) * u[j];
-      }
-      *reinterpret_cast<uint4*>(gu + f) = pack8(a);
-      *reinterpret_cast<uint4*>(gu + F + f) = pack8(u);
-      *reinterpret_cast<uint4*>(ao + f) = pack8(o);
-    }
-  }
-}
-
 template <int BN, bool A_MN, bool B_MN, int ACT>
-__global__ void __launch_bounds__(320, 1)
-gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const __grid_constant__ CUtensorMap tmC, int M, int N, int K, int batch, GemmEpilogue ep) {
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K,
+                GemmEpilogue ep) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
+  constexpr bool SWIGLU = ACT == ACT_SWIGLU_PAIR;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte aligned bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
-  // barrier layout: full[STAGES], empty[STAGES], tmem_full[2], tmem_empty[2], tmem slot
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-
+  // SwiGLU: N = 2F columns, one tile = 64 features (64 gate + 64 up columns)
   const int m_blocks = (M + BM - 1) / BM;
-  const int n_blocks = (N + BN - 1) / BN;
+  const int n_blocks = SWIGLU ? (N / 2) / 64 : (N + BN - 1) / BN;
   const int tiles_per_batch = m_blocks * n_blocks;
-  const int num_tiles = tiles_per_batch * batch;
+  const int b = blockIdx.x / tiles_per_batch;
+  int mb, nb;
+  tile_to_mn(blockIdx.x - b * tiles_per_batch, m_blocks, n_blocks, mb, nb);
+  const int m0 = mb * BM;
   const int num_kb = (K + BK - 1) / BK;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 2);  // one arrive per consumer warpgroup
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), 8);  // one arrive per epilogue warp
-    }
-    ring_init(make_ring(bar_base));
     mbar_fence_init();
   }
-  const TileRing ring = make_ring(bar_base);
-  const bool dyn = ep.dyn != 0;
-  if (warp == 1) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ============================ TMA producer ============================
     if (lane == 0) {
       int stage = 0;
-      uint32_t phase = 0, clc_phase = 0;
-      int it = 0;
-      int tile = blockIdx.x;
-      while (true) {
-        if (dyn) ring_publish(ring, it, tile);
-        if (tile < 0) break;
-        if (dyn) {  // ask for the next tile now; the answer arrives while this tile's operands stream in
-          mbar_arrive_expect_tx(ring.clc_bar, 16);
-          clc_try_cancel(ring.resp, ring.clc_bar);
-        }
-        const int b = tile / tiles_per_batch;
-        const int r = tile - b * tiles_per_batch;
-        int mb_, nb_;
-        tile_to_mn(r, m_blocks, n_blocks, ep.group_m, mb_, nb_);
-        const int m0 = mb_ * BM;
-        const int n0 = nb_ * BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
-          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint32_t sb = sa + Cfg::A_BYTES;
-          mbar_arrive_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
-          const int k0 = kb * BK;
-          if (!A_MN) {
-            tma_load_3d(sa, &tmA, full_bar(stage), k0, m0, b);
-          } else {
-#pragma unroll
-            for (int i = 0; i < BM / 64; ++i)
-              tma_load_3d(sa + i * (64 * BK * 2), &tmA, full_bar(stage), m0 + 64 * i, k0, b);
-          }
-          if (!B_MN) {
-            tma_load_3d(sb, &tmB, full_bar(stage), k0, n0, b);
-          } else {
-#pragma unroll
-            for (int i = 0; i < BN / 64; ++i)
-              tma_load_3d(sb + i * (64 * BK * 2), &tmB, full_bar(stage), n0 + 64 * i, k0, b);
-          }
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        if (dyn) {
-          mbar_wait(ring.clc_bar, clc_phase);
-          clc_phase ^= 1u;
-          tile = clc_decode(ring.resp);  // blockIdx.x of the cancelled CTA == its tile; -1: the grid is exhausted
-          ++it;
+      uint32_t phase = 0;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(empty_bar(stage), phase ^ 1u);
+        const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
+        const uint32_t sb = sa + Cfg::A_BYTES;
+        mbar_arrive_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
+        const int k0 = kb * BK;
+        if (!A_MN) {
+          tma_load_3d(sa, &tmA, full_bar(stage), k0, m0, b);
         } else {
-          tile += gridDim.x;
-          if (tile >= num_tiles) break;
+#pragma unroll
+          for (int i = 0; i < BM / 64; ++i) tma_load_3d(sa + i * (64 * BK * 2), &tmA, full_bar(stage), m0 + 64 * i, k0, b);
+        }
+        if (SWIGLU) {  // gate rows [64 nb, +64) and up rows [F + 64 nb, +64)
+          tma_load_3d(sb, &tmB, full_bar(stage), k0, nb * 64, 0);
+          tma_load_3d(sb + 64 * BK * 2, &tmB, full_bar(stage), k0, N / 2 + nb * 64, 0);
+        } else if (!B_MN) {
+          tma_load_3d(sb, &tmB, full_bar(stage), k0, nb * BN, b);
+        } else {
+#pragma unroll
+          for (int i = 0; i < BN / 64; ++i)
+            tma_load_3d(sb + i * (64 * BK * 2), &tmB, full_bar(stage), nb * BN + 64 * i, k0, b);
+        }
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1u;
         }
       }
     }
-  } else if (warp == 1) {
-    // ============================ MMA issuer ==============================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(BM, BN, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      int it = 0;
-      for (int tile = dyn ? ring_fetch(ring, 0) : (int)blockIdx.x; tile >= 0 && tile < num_tiles;
-           tile = dyn ? ring_fetch(ring, ++it) : tile + (int)gridDim.x) {
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * BN);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint32_t sb = sa + Cfg::A_BYTES;
+    return;
+  }
+
+  // ============================ consumer warpgroups ============================
+  const int wg = warp >> 2;  // rows [64 wg, +64) of the tile
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  float acc[BN / 2];
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t adesc = A_MN ? make_smem_desc_sw128(sa + k * 2048, 64 * BK * 2, 1024)
-                                        : make_smem_desc_sw128(sa + k * 32, 0, 1024);
-            const uint64_t bdesc = B_MN ? make_smem_desc_sw128(sb + k * 2048, 64 * BK * 2, 1024)
-                                        : make_smem_desc_sw128(sb + k * 32, 0, 1024);
-            umma_ss(d_tmem, adesc, bdesc, idesc, (kb | k) ? 1u : 0u);
-          }
-          umma_commit(empty_bar(stage));  // smem slot is free once these MMAs retire
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        umma_commit(tfull_bar(acc));  // accumulator complete -> epilogue
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1u;
-        }
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  int stage = 0;
+  uint32_t phase = 0;
+  int prev_stage = -1;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait(full_bar(stage), phase);
+    const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES + wg * (64 * 128);
+    const uint32_t sb = smem_base + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES;
+    reg_fence(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+      const uint64_t adesc = A_MN ? make_smem_desc_sw128(sa + k * 2048, 64 * BK * 2, 1024)
+                                  : make_smem_desc_sw128(sa + k * 32, 0, 1024);
+      const uint64_t bdesc = B_MN ? make_smem_desc_sw128(sb + k * 2048, 64 * BK * 2, 1024)
+                                  : make_smem_desc_sw128(sb + k * 32, 0, 1024);
+      WgmmaSS<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>::mma(acc, adesc, bdesc, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage can be refilled
+    reg_fence(acc);
+    if (prev_stage >= 0 && wg_leader) mbar_arrive(empty_bar(prev_stage));
+    prev_stage = stage;
+    if (++stage == STAGES) {
+      stage = 0;
+      phase ^= 1u;
+    }
+  }
+  wgmma_wait<0>();
+  reg_fence(acc);
+
+  // ============================ epilogue ============================
+  const int r_lo = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  if constexpr (SWIGLU) {
+    // accumulator columns [0, 64) = gate, [64, 128) = up of the same 64 features: write both pre-activations (saved for
+    // backward) and silu(gate) * up without a second pass over the [M, 2F] tensor
+    const int F = N >> 1;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r_lo + 8 * h;
+      if (row >= M) continue;
+      bf16* gu = reinterpret_cast<bf16*>(ep.C) + static_cast<long long>(row) * ep.ldc;
+      bf16* ao = reinterpret_cast<bf16*>(ep.aux) + static_cast<long long>(row) * ep.ld_aux;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int f = nb * 64 + 8 * j + cq;
+        // round to bf16 first: the separate kernels (and the reference) apply silu to the STORED bf16 pre-activations
+        const __nv_bfloat162 g2 = __floats2bfloat162_rn(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        const __nv_bfloat162 u2 = __floats2bfloat162_rn(acc[4 * (j + 8) + 2 * h], acc[4 * (j + 8) + 2 * h + 1]);
+        const float2 g = __bfloat1622float2(g2), u = __bfloat1622float2(u2);
+        *reinterpret_cast<__nv_bfloat162*>(gu + f) = g2;
+        *reinterpret_cast<__nv_bfloat162*>(gu + F + f) = u2;
+        *reinterpret_cast<__nv_bfloat162*>(ao + f) = __floats2bfloat162_rn(silu(g.x) * u.x, silu(g.y) * u.y);
       }
     }
   } else {
-    // ============================ epilogue ================================
-    const int lane_grp = warp & 3;  // TMEM lanes [32*lane_grp, +32) are accessible to this warp
-    const int col_half = (warp - 2) >> 2;  // warps 2-5: first half of the tile's columns, warps 6-9: second half
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    StageRing sring{bar_base + 1024u + static_cast<uint32_t>(warp - 2) * 4096u, 0};
-    int it = 0;
-    for (int tile = dyn ? ring_fetch_warp(ring, 0, lane) : (int)blockIdx.x; tile >= 0 && tile < num_tiles;
-         tile = dyn ? ring_fetch_warp(ring, ++it, lane) : tile + (int)gridDim.x) {
-      const int b = tile / tiles_per_batch;
-      const int r = tile - b * tiles_per_batch;
-      int mb_, nb_;
-      tile_to_mn(r, m_blocks, n_blocks, ep.group_m, mb_, nb_);
-      const int m0 = mb_ * BM;
-      const int n0 = nb_ * BN;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      const int row = m0 + lane_grp * 32 + lane;
-      const bool row_ok = row < M;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(lane_grp * 32) << 16) +
-                             static_cast<uint32_t>(acc * BN);
-      epilogue_columns<BN, ACT>(ep, taddr, row, row_ok, b, n0, N, col_half * (BN / 64), sring, &tmC,
-                                m0 + lane_grp * 32, lane);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1u;
+    const int n0 = nb * BN;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r_lo + 8 * h;
+      if (row >= M) continue;
+      const long long c_off = static_cast<long long>(b) * ep.bsc + static_cast<long long>(row) * ep.ldc;
+      const long long r_off = static_cast<long long>(b) * ep.bsr + static_cast<long long>(row) * ep.ldr;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = n0 + 8 * j + cq;
+        if (n0 + 8 * j >= N) break;
+        epilogue_pair<ACT>(ep, c_off, r_off, col, N, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
       }
     }
   }
-
-  if (warp >= 2 && lane == 0) bulk_wait_group0();  // staged output tiles fully written before the CTA retires
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 1) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-}
-
-// ------------------------------------------------------------------------------------------
-// CTA-pair variant (cta_group::2): a (2,1,1) cluster computes one 256 x BN tile.  Each CTA stages its own 128 rows of
-// A and HALF of the B tile (BN/2 rows), so the operand bytes streamed into and read out of each SM's shared memory per
-// FLOP drop by a third versus the 128 x BN single-CTA tile — the shared-memory port, not the tensor pipe, bounds the
-// single-CTA kernel at ~65% utilisation under the power cap.  The leader CTA's MMA warp issues tcgen05.mma.cta_group::2
-// (M = 256); both CTAs' TMA loads credit the leader's `full` barrier; tcgen05.commit multicasts to both CTAs' `empty` /
-// `tmem_full` barriers; both CTAs' epilogue warps arrive on the leader's `tmem_empty` barrier.
-// ------------------------------------------------------------------------------------------
-template <int BN>
-struct Gemm2Cfg {
-  static constexpr int HALF_N = BN / 2;
-  static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = HALF_N * BK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BN == 256) ? 6 : 8;
-  static constexpr int TMEM_COLS = 2 * BN;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 1024 + 32768;  // align slack, barriers, store staging
-};
-
-template <int BN, bool A_MN, bool B_MN, int ACT>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(320, 1)
-gemm_bf16_tcgen05_2cta(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                       const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAux, int M, int N,
-                       int K, int batch, GemmEpilogue ep) {
-  using Cfg = Gemm2Cfg<BN>;
-  constexpr int STAGES = Cfg::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-
-  const int m_blocks = (M + 2 * BM - 1) / (2 * BM);
-  const int n_blocks = (N + BN - 1) / BN;
-  const int tiles_per_batch = m_blocks * n_blocks;
-  const int num_tiles = tiles_per_batch * batch;
-  const int num_kb = (K + BK - 1) / BK;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1);   // leader's copy is the one in use: its own arrive.expect_tx, bytes from both CTAs
-      mbar_init(empty_bar(s), 1);  // multicast commit from the leader's MMA thread
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), 16);  // 8 epilogue warps x 2 CTAs arrive on the leader's copy
-    }
-    ring_init(make_ring(bar_base));
-    mbar_fence_init();
-  }
-  const TileRing ring = make_ring(bar_base);
-  const bool dyn = ep.dyn != 0;
-  if (warp == 1) tmem_alloc_2cta(tmem_slot, Cfg::TMEM_COLS);
-  tc_fence_before();
-  cluster_sync_all();  // barrier inits + TMEM allocation of both CTAs visible before any cross-CTA traffic
-  __syncthreads();     // (the cluster barrier already orders this; a CTA barrier is what compute-sanitizer racecheck models
-                       //  between tcgen05.alloc's shared-memory write and the read below — one-time cost)
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-
-  if (warp == 0) {
-    // ============================ TMA producer (both CTAs) ============================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0, clc_phase = 0;
-      int it = 0;
-      int tile = cluster_id;
-      while (true) {
-        if (dyn) ring_publish(ring, it, tile);  // each CTA's producer feeds its own CTA's MMA / epilogue warps
-        if (tile < 0) break;
-        if (dyn) {
-          // one query per cluster, issued by the leader, answered into BOTH CTAs' response slot / barrier (multicast);
-          // every CTA arms its own barrier.  The slot is single-buffered: the leader waits until the peer has decoded the
-          // previous answer (clc_empty, remote arrive below) before it lets the next one land.
-          mbar_arrive_expect_tx(ring.clc_bar, 16);
-          if (leader) {
-            if (it > 0) mbar_wait(ring.clc_empty, static_cast<uint32_t>((it - 1) & 1));
-            clc_try_cancel_multicast(ring.resp, ring.clc_bar);
-          }
-        }
-        const int b = tile / tiles_per_batch;
-        const int r = tile - b * tiles_per_batch;
-        int mb_, nb_;
-        tile_to_mn(r, m_blocks, n_blocks, ep.group_m, mb_, nb_);
-        const int m0 = mb_ * (2 * BM) + static_cast<int>(rank) * BM;
-        const int n0 = (ACT == ACT_SWIGLU_PAIR) ? nb_ * Cfg::HALF_N + static_cast<int>(rank) * (N >> 1)
-                                                : nb_ * BN + static_cast<int>(rank) * Cfg::HALF_N;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
-          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint32_t sb = sa + Cfg::A_BYTES;
-          if (leader) mbar_arrive_expect_tx(full_bar(stage), 2 * Cfg::STAGE_BYTES);
-          const int k0 = kb * BK;
-          if (!A_MN) {
-            tma_load_3d_2cta(sa, &tmA, full_bar(stage), k0, m0, b);
-          } else {
-#pragma unroll
-            for (int i = 0; i < BM / 64; ++i)
-              tma_load_3d_2cta(sa + i * (64 * BK * 2), &tmA, full_bar(stage), m0 + 64 * i, k0, b);
-          }
-          if (!B_MN) {
-            tma_load_3d_2cta(sb, &tmB, full_bar(stage), k0, n0, b);
-          } else {
-#pragma unroll
-            for (int i = 0; i < Cfg::HALF_N / 64; ++i)
-              tma_load_3d_2cta(sb + i * (64 * BK * 2), &tmB, full_bar(stage), n0 + 64 * i, k0, b);
-          }
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        if (dyn) {
-          mbar_wait(ring.clc_bar, clc_phase);
-          clc_phase ^= 1u;
-          const int x = clc_decode(ring.resp);  // blockIdx.x of the cancelled cluster's first CTA
-          tile = x < 0 ? -1 : (x >> 1);
-          if (!leader) mbar_arrive_cluster(ring.clc_empty, 0);
-          ++it;
-        } else {
-          tile += num_clusters;
-          if (tile >= num_tiles) break;
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ============================ MMA issuer (leader CTA only) ========================
-    if (!leader && lane == 0 && dyn) {
-      // the peer's MMA warp has no MMAs to issue; it only takes its share of the ring's `empty` arrivals
-      for (int it = 0; ring_fetch(ring, it) >= 0; ++it) {
-      }
-    }
-    if (leader && lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(2 * BM, BN, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      int it = 0;
-      for (int tile = dyn ? ring_fetch(ring, 0) : cluster_id; tile >= 0 && tile < num_tiles;
-           tile = dyn ? ring_fetch(ring, ++it) : tile + num_clusters) {
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * BN);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint32_t sb = sa + Cfg::A_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t adesc = A_MN ? make_smem_desc_sw128(sa + k * 2048, 64 * BK * 2, 1024)
-                                        : make_smem_desc_sw128(sa + k * 32, 0, 1024);
-            const uint64_t bdesc = B_MN ? make_smem_desc_sw128(sb + k * 2048, 64 * BK * 2, 1024)
-                                        : make_smem_desc_sw128(sb + k * 32, 0, 1024);
-            umma_ss_2cta(d_tmem, adesc, bdesc, idesc, (kb | k) ? 1u : 0u);
-          }
-          umma_commit_2cta_mc(empty_bar(stage), 3);  // frees the slot in BOTH CTAs
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        umma_commit_2cta_mc(tfull_bar(acc), 3);  // accumulator halves complete in both CTAs' TMEM
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1u;
-        }
-      }
-    }
-  } else {
-    // ============================ epilogue (both CTAs, own 128 rows) ==================
-    const int lane_grp = warp & 3;
-    const int col_half = (warp - 2) >> 2;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    StageRing sring{bar_base + 1024u + static_cast<uint32_t>(warp - 2) * 4096u, 0};
-    int it = 0;
-    for (int tile = dyn ? ring_fetch_warp(ring, 0, lane) : cluster_id; tile >= 0 && tile < num_tiles;
-         tile = dyn ? ring_fetch_warp(ring, ++it, lane) : tile + num_clusters) {
-      const int b = tile / tiles_per_batch;
-      const int r = tile - b * tiles_per_batch;
-      int mb_, nb_;
-      tile_to_mn(r, m_blocks, n_blocks, ep.group_m, mb_, nb_);
-      const int m0 = mb_ * (2 * BM) + static_cast<int>(rank) * BM;
-      const int n0 = nb_ * BN;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      const int row = m0 + lane_grp * 32 + lane;
-      const bool row_ok = row < M;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(lane_grp * 32) << 16) +
-                             static_cast<uint32_t>(acc * BN);
-      if constexpr (ACT == ACT_SWIGLU_PAIR)
-        epilogue_swiglu_pair(ep, taddr, row, row_ok, nb_, N, col_half, sring, &tmC, &tmAux, m0 + lane_grp * 32, lane);
-      else
-        epilogue_columns<BN, ACT>(ep, taddr, row, row_ok, b, n0, N, col_half * (BN / 64), sring, &tmC,
-                                  m0 + lane_grp * 32, lane);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(tempty_bar(acc), 0);  // leader's barrier
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1u;
-      }
-    }
-  }
-
-  if (warp >= 2 && lane == 0) bulk_wait_group0();  // staged output tiles fully written before the CTA retires
-  tc_fence_before();
-  cluster_sync_all();  // the leader's MMAs read the peer's smem: nobody may exit (or free TMEM) before both are done
-  tc_fence_after();
-  if (warp == 1) tmem_dealloc_2cta(tmem_base, Cfg::TMEM_COLS);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -871,132 +337,40 @@ int make_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t inner, uint64
   return CB_OK;
 }
 
-// bf16 output [batch, rows, cols] (ld elements per row): 32 x 32 store boxes, SWIZZLE_64B (see StageRing)
-static int make_tmap_out(CUtensorMap* out, void* base, uint64_t cols, uint64_t rows, uint64_t batch, uint64_t ld_elems,
-                         uint64_t batch_stride_elems) {
-  auto fn = get_encode_fn();
-  if (!fn) return set_error(CB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t dims[3] = {cols, rows, batch};
-  cuuint64_t bs = (batch > 1) ? batch_stride_elems * 2 : ld_elems * 2 * (rows ? rows : 1);
-  cuuint64_t strides[2] = {ld_elems * 2, bs};
-  cuuint32_t box[3] = {32, 32, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = CUDA_SUCCESS;
-  for (int attempt = 0; attempt < 2; ++attempt) {
-    r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_ERROR_INVALID_CONTEXT) break;
-    cudaFree(0);
-  }
-  if (r != CUDA_SUCCESS) return set_error(CB_ERR_CUDA, "cuTensorMapEncodeTiled(out) failed (%d)", (int)r);
-  return CB_OK;
-}
-
-static bool tma_store_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("CB_GEMM_TMA_STORE");
-    on = (e && e[0] == '0') ? 0 : 1;
-  }
-  return on == 1;
-}
-
 template <int BN, bool A_MN, bool B_MN, int ACT>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, int M, int N, int K,
-                       int batch, const GemmEpilogue& ep, cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, int batch,
+                       const GemmEpilogue& ep, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_bf16_tcgen05<BN, A_MN, B_MN, ACT>;
+  auto kern = gemm_bf16_wgmma<BN, A_MN, B_MN, ACT>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
     if (e != cudaSuccess) return set_error(CB_ERR_CUDA, "gemm smem attr: %s", cudaGetErrorString(e));
     attr_set = true;
   }
-  const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN) * batch;
-  const int grid = (ep.dyn || tiles < device_sm_count()) ? tiles : device_sm_count();
-  kern<<<grid, 320, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmC, M, N, K, batch, ep);
-  CB_CUDA_LAUNCH_CHECK("gemm_bf16_tcgen05");
+  const int n_blocks = (ACT == ACT_SWIGLU_PAIR) ? (N / 2) / 64 : (N + BN - 1) / BN;
+  const long long tiles = (long long)((M + BM - 1) / BM) * n_blocks * batch;
+  CB_CHECK_ARG(tiles < (1LL << 31), "gemm: %lld tiles exceed the grid", tiles);
+  kern<<<(unsigned)tiles, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, M, N, K, ep);
+  CB_CUDA_LAUNCH_CHECK("gemm_bf16_wgmma");
   return CB_OK;
-}
-
-template <int BN, bool A_MN, bool B_MN, int ACT>
-static int launch_gemm2(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmAux,
-                        int M, int N, int K, int batch, const GemmEpilogue& ep, cudaStream_t stream) {
-  using Cfg = Gemm2Cfg<BN>;
-  auto kern = gemm_bf16_tcgen05_2cta<BN, A_MN, B_MN, ACT>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return set_error(CB_ERR_CUDA, "gemm2 smem attr: %s", cudaGetErrorString(e));
-    attr_set = true;
-  }
-  const int tiles = ((M + 2 * BM - 1) / (2 * BM)) * ((N + BN - 1) / BN) * batch;
-  const int pairs = device_sm_count() / 2;
-  const int clusters = (ep.dyn || tiles < pairs) ? tiles : pairs;
-  kern<<<2 * clusters, 320, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmC, tmAux, M, N, K, batch, ep);
-  CB_CUDA_LAUNCH_CHECK("gemm_bf16_tcgen05_2cta");
-  return CB_OK;
-}
-
-static int dispatch_2cta(int a_mn, int b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, int M,
-                         int N, int K,
-                         int batch, const GemmEpilogue& ep, cudaStream_t stream) {
-  if (!a_mn && !b_mn) {  // forward layout: the only one that carries a fused activation
-    switch (ep.act) {
-      case 1: return launch_gemm2<256, false, false, 1>(tmA, tmB, tmC, tmC, M, N, K, batch, ep, stream);
-      case 2: return launch_gemm2<256, false, false, 2>(tmA, tmB, tmC, tmC, M, N, K, batch, ep, stream);
-      case 3: return launch_gemm2<256, false, false, 3>(tmA, tmB, tmC, tmC, M, N, K, batch, ep, stream);
-      case 4: return launch_gemm2<256, false, false, 4>(tmA, tmB, tmC, tmC, M, N, K, batch, ep, stream);
-      default: return launch_gemm2<256, false, false, 0>(tmA, tmB, tmC, tmC, M, N, K, batch, ep, stream);
-    }
-  }
-  if (!a_mn && b_mn) return launch_gemm2<256, false, true, 0>(tmA, tmB, tmC, tmC, M, N, K, batch, ep, stream);
-  if (a_mn && !b_mn) return launch_gemm2<256, true, false, 0>(tmA, tmB, tmC, tmC, M, N, K, batch, ep, stream);
-  return launch_gemm2<256, true, true, 0>(tmA, tmB, tmC, tmC, M, N, K, batch, ep, stream);
-}
-
-// CB_GEMM_CLC=0 keeps the static persistent tile walk (read once); default: dynamic scheduling through Cluster Launch
-// Control whenever a GEMM has more tiles than one wave
-static int g_clc = -1;
-static bool clc_enabled() {
-  if (g_clc < 0) {
-    const char* e = getenv("CB_GEMM_CLC");
-    g_clc = (e && e[0] == '0') ? 0 : 1;
-  }
-  return g_clc == 1;
-}
-int gemm_set_dynamic_scheduling(int on) {  // returns the previous setting (A/B comparisons inside one process)
-  const int prev = clc_enabled() ? 1 : 0;
-  g_clc = on ? 1 : 0;
-  return prev;
-}
-
-// CB_GEMM_2CTA=0 disables the CTA-pair kernel (read once)
-static bool two_cta_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("CB_GEMM_2CTA");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
 }
 
 template <int BN>
-static int dispatch_major(int a_mn, int b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, int M,
-                          int N,
+static int dispatch_major(int a_mn, int b_mn, int act, const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N,
                           int K, int batch, const GemmEpilogue& ep, cudaStream_t stream) {
   if (!a_mn && !b_mn) {
-    switch (ep.act) {
-      case 1: return launch_gemm<BN, false, false, 1>(tmA, tmB, tmC, M, N, K, batch, ep, stream);
-      case 2: return launch_gemm<BN, false, false, 2>(tmA, tmB, tmC, M, N, K, batch, ep, stream);
-      case 3: return launch_gemm<BN, false, false, 3>(tmA, tmB, tmC, M, N, K, batch, ep, stream);
-      case 4: return launch_gemm<BN, false, false, 4>(tmA, tmB, tmC, M, N, K, batch, ep, stream);
-      default: return launch_gemm<BN, false, false, 0>(tmA, tmB, tmC, M, N, K, batch, ep, stream);
+    switch (act) {
+      case 1: return launch_gemm<BN, false, false, 1>(tmA, tmB, M, N, K, batch, ep, stream);
+      case 2: return launch_gemm<BN, false, false, 2>(tmA, tmB, M, N, K, batch, ep, stream);
+      case 3: return launch_gemm<BN, false, false, 3>(tmA, tmB, M, N, K, batch, ep, stream);
+      case 4: return launch_gemm<BN, false, false, 4>(tmA, tmB, M, N, K, batch, ep, stream);
+      default: return launch_gemm<BN, false, false, 0>(tmA, tmB, M, N, K, batch, ep, stream);
     }
   }
-  if (!a_mn && b_mn) return launch_gemm<BN, false, true, 0>(tmA, tmB, tmC, M, N, K, batch, ep, stream);
-  if (a_mn && !b_mn) return launch_gemm<BN, true, false, 0>(tmA, tmB, tmC, M, N, K, batch, ep, stream);
-  return launch_gemm<BN, true, true, 0>(tmA, tmB, tmC, M, N, K, batch, ep, stream);
+  if (!a_mn && b_mn) return launch_gemm<BN, false, true, 0>(tmA, tmB, M, N, K, batch, ep, stream);
+  if (a_mn && !b_mn) return launch_gemm<BN, true, false, 0>(tmA, tmB, M, N, K, batch, ep, stream);
+  return launch_gemm<BN, true, true, 0>(tmA, tmB, M, N, K, batch, ep, stream);
 }
 
 int gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int batch, long long lda,
@@ -1008,18 +382,11 @@ int gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int ba
   CB_CHECK_ARG(A && B && C, "gemm: null operand");
   CB_CHECK_ARG(act >= 0 && act <= 4, "gemm: unknown activation %d", act);
   CB_CHECK_ARG(act == 0 || (!a_mn && !b_mn), "gemm: a fused activation needs K-major operands (forward layout)");
-  CUtensorMap tmA, tmB;
-  int rc;
+  CB_CHECK_ARG(force_bn == 0 || force_bn == 64 || force_bn == 128 || force_bn == 256, "gemm: bad BLOCK_N %d", force_bn);
   int bn = force_bn;
-  // force_bn = 512 selects the CTA-pair (256 x 256 per cluster) kernel explicitly; the heuristic picks it for problems
-  // that fill the 74 SM pairs for at least ~3 waves (the large decoder / lm_head / ConvNeXt GEMMs)
-  bool use_2cta = (force_bn == 512);
-  if (force_bn == 0 && two_cta_enabled() && N >= 256) {
-    const long long t2 = (long long)((M + 2 * BM - 1) / (2 * BM)) * ((N + 255) / 256) * batch;
-    if (t2 >= 3LL * (device_sm_count() / 2)) use_2cta = true;
-  }
-  if (use_2cta) bn = 256;
   if (bn == 0) {
+    // the widest tile that still gives most SMs a CTA: wide tiles halve the operand traffic per FLOP, but a GEMM of
+    // fewer tiles than SMs leaves the rest of the chip idle
     const int sms = device_sm_count();
     const long long mb = (M + BM - 1) / BM;
     auto tiles = [&](int b_n) { return mb * ((N + b_n - 1) / b_n) * batch; };
@@ -1028,11 +395,12 @@ int gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int ba
     else if (N > 128 && tiles(64) > 2LL * sms) bn = 128;
     else bn = 64;
   }
-  CB_CHECK_ARG(bn == 64 || bn == 128 || bn == 256, "gemm: bad BLOCK_N %d", bn);
+  CUtensorMap tmA, tmB;
+  int rc;
   if (!a_mn) rc = make_tmap_bf16_3d(&tmA, A, K, M, batch, lda, bsa, BM);
   else       rc = make_tmap_bf16_3d(&tmA, A, M, K, batch, lda, bsa, BK);
   if (rc) return rc;
-  if (!b_mn) rc = make_tmap_bf16_3d(&tmB, B, K, N, batch, ldb, bsb, use_2cta ? bn / 2 : bn);
+  if (!b_mn) rc = make_tmap_bf16_3d(&tmB, B, K, N, batch, ldb, bsb, bn);
   else       rc = make_tmap_bf16_3d(&tmB, B, N, K, batch, ldb, bsb, BK);
   if (rc) return rc;
   GemmEpilogue ep;
@@ -1041,52 +409,29 @@ int gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int ba
   ep.colscale = static_cast<const bf16*>(colscale);
   ep.residual = static_cast<const bf16*>(residual);
   ep.ldr = ldr; ep.bsr = bsr;
-  ep.alpha = alpha; ep.act = act; ep.out_fp32 = out_fp32; ep.accumulate = accumulate;
+  ep.alpha = alpha; ep.out_fp32 = out_fp32; ep.accumulate = accumulate;
   ep.aux = nullptr; ep.ld_aux = 0;
-  {
-    // dynamic scheduling only pays (and only differs) when the static grid would be persistent: more tiles than SMs
-    const long long t = use_2cta ? (long long)((M + 2 * BM - 1) / (2 * BM)) * ((N + bn - 1) / bn) * batch * 2
-                                 : (long long)((M + BM - 1) / BM) * ((N + bn - 1) / bn) * batch;
-    ep.dyn = (clc_enabled() && t > device_sm_count()) ? 1 : 0;
-  }
-  const int cvec = out_fp32 ? 4 : 8;
-  bool vec = (N % 8 == 0) && (ldc % cvec == 0) && (bsc % cvec == 0) &&
-             ((reinterpret_cast<uintptr_t>(C) & 15u) == 0);
+  const unsigned calign = out_fp32 ? 7u : 3u;
+  bool pair = (N % 2 == 0) && (ldc % 2 == 0) && (bsc % 2 == 0) && ((reinterpret_cast<uintptr_t>(C) & calign) == 0);
   if (residual)
-    vec = vec && (ldr % 8 == 0) && (bsr % 8 == 0) && ((reinterpret_cast<uintptr_t>(residual) & 15u) == 0);
-  if (bias) vec = vec && ((reinterpret_cast<uintptr_t>(bias) & 15u) == 0);
-  if (colscale) vec = vec && ((reinterpret_cast<uintptr_t>(colscale) & 15u) == 0);
-  ep.vec_ok = vec ? 1 : 0;
-  CUtensorMap tmC;
-  memset(&tmC, 0, sizeof(tmC));
-  ep.tma_store = 0;
-  if (vec && !out_fp32 && !accumulate && tma_store_enabled()) {
-    if ((rc = make_tmap_out(&tmC, C, N, M, batch, ldc, bsc))) return rc;
-    ep.tma_store = 1;
-  }
-  {
-    static int gm = -1;  // CB_GEMM_GROUP_M: rows of the L2 super-row (default 2048 rows)
-    if (gm < 0) {
-      const char* e = getenv("CB_GEMM_GROUP_M");
-      gm = e ? atoi(e) : 2048;
-    }
-    ep.group_m = gm / (use_2cta ? 2 * BM : BM);
-  }
-  if (use_2cta) return dispatch_2cta(a_mn, b_mn, tmA, tmB, tmC, M, N, K, batch, ep, stream);
+    pair = pair && (ldr % 2 == 0) && (bsr % 2 == 0) && ((reinterpret_cast<uintptr_t>(residual) & 3u) == 0);
+  if (bias) pair = pair && ((reinterpret_cast<uintptr_t>(bias) & 3u) == 0);
+  if (colscale) pair = pair && ((reinterpret_cast<uintptr_t>(colscale) & 3u) == 0);
+  ep.pair_ok = pair ? 1 : 0;
   switch (bn) {
-    case 256: return dispatch_major<256>(a_mn, b_mn, tmA, tmB, tmC, M, N, K, batch, ep, stream);
-    case 128: return dispatch_major<128>(a_mn, b_mn, tmA, tmB, tmC, M, N, K, batch, ep, stream);
-    default:  return dispatch_major<64>(a_mn, b_mn, tmA, tmB, tmC, M, N, K, batch, ep, stream);
+    case 256: return dispatch_major<256>(a_mn, b_mn, act, tmA, tmB, M, N, K, batch, ep, stream);
+    case 128: return dispatch_major<128>(a_mn, b_mn, act, tmA, tmB, M, N, K, batch, ep, stream);
+    default:  return dispatch_major<64>(a_mn, b_mn, act, tmA, tmB, M, N, K, batch, ep, stream);
   }
 }
 
-// gate/up projection + SwiGLU in one CTA-pair GEMM.  A [M, K] (lda), W = [gate_proj; up_proj] [2F, K] (ldw);
+// gate/up projection + SwiGLU in one GEMM.  A [M, K] (lda), W = [gate_proj; up_proj] [2F, K] (ldw);
 // gu_out [M, 2F] (ld_gu) receives the bf16 pre-activations, act_out [M, F] (ld_act) silu(gate) * up.
 int gemm_swiglu_bf16(const void* A, const void* W, void* gu_out, void* act_out, int M, int F, int K, long long lda,
                      long long ldw, long long ld_gu, long long ld_act, cudaStream_t stream) {
   CB_CHECK_ARG(M > 0 && F > 0 && K > 0, "gemm_swiglu: empty problem M=%d F=%d K=%d", M, F, K);
   CB_CHECK_ARG(A && W && gu_out && act_out, "gemm_swiglu: null operand");
-  CB_CHECK_ARG(F % 128 == 0, "gemm_swiglu: F=%d must be a multiple of 128 (one tile pairs 128 gate with 128 up columns)", F);
+  CB_CHECK_ARG(F % 128 == 0, "gemm_swiglu: F=%d must be a multiple of 128 (whole 64-feature tiles, 16-byte aligned halves)", F);
   CB_CHECK_ARG(ld_gu % 8 == 0 && ld_act % 8 == 0 && ((reinterpret_cast<uintptr_t>(gu_out) & 15u) == 0) &&
                    ((reinterpret_cast<uintptr_t>(act_out) & 15u) == 0),
                "gemm_swiglu: outputs must be 16-byte aligned with ld %% 8 == 0");
@@ -1094,29 +439,13 @@ int gemm_swiglu_bf16(const void* A, const void* W, void* gu_out, void* act_out, 
   CUtensorMap tmA, tmB;
   int rc;
   if ((rc = make_tmap_bf16_3d(&tmA, A, K, M, 1, lda, 0, BM))) return rc;
-  if ((rc = make_tmap_bf16_3d(&tmB, W, K, N, 1, ldw, 0, 128))) return rc;
+  if ((rc = make_tmap_bf16_3d(&tmB, W, K, N, 1, ldw, 0, 64))) return rc;
   GemmEpilogue ep;
   ep.C = gu_out; ep.ldc = ld_gu; ep.bsc = 0;
   ep.bias = nullptr; ep.colscale = nullptr; ep.residual = nullptr; ep.ldr = 0; ep.bsr = 0;
-  ep.alpha = 1.0f; ep.act = ACT_SWIGLU_PAIR; ep.out_fp32 = 0; ep.accumulate = 0; ep.vec_ok = 1;
+  ep.alpha = 1.0f; ep.out_fp32 = 0; ep.accumulate = 0; ep.pair_ok = 1;
   ep.aux = act_out; ep.ld_aux = ld_act;
-  ep.dyn = (clc_enabled() && 2LL * ((M + 2 * BM - 1) / (2 * BM)) * (N / 256) > device_sm_count()) ? 1 : 0;
-  CUtensorMap tmC, tmAux;
-  memset(&tmC, 0, sizeof(tmC));
-  memset(&tmAux, 0, sizeof(tmAux));
-  ep.tma_store = 0;
-  if (tma_store_enabled()) {
-    if ((rc = make_tmap_out(&tmC, gu_out, N, M, 1, ld_gu, 0))) return rc;
-    if ((rc = make_tmap_out(&tmAux, act_out, F, M, 1, ld_act, 0))) return rc;
-    ep.tma_store = 1;
-  }
-  static int gm = -1;
-  if (gm < 0) {
-    const char* e = getenv("CB_GEMM_GROUP_M");
-    gm = e ? atoi(e) : 2048;
-  }
-  ep.group_m = gm / (2 * BM);
-  return launch_gemm2<256, false, false, ACT_SWIGLU_PAIR>(tmA, tmB, tmC, tmAux, M, N, K, 1, ep, stream);
+  return launch_gemm<128, false, false, ACT_SWIGLU_PAIR>(tmA, tmB, M, N, K, 1, ep, stream);
 }
 
 }  // namespace cb

@@ -1,9 +1,8 @@
 // cambrian_b200 — weight-streaming GEMV for decode-shaped projections (M <= 8 rows: one token per sequence of a generate()
 // batch, cambrian_llama.py:437-483 -> HF greedy loop).   y[M, N] = x[M, K] W[N, K]^T (+ bias) (+ residual)
 //
-// With <= 8 rows the 128-row tcgen05 tile wastes > 93 % of the tensor pipe and, worse, streams the weights at a fraction of
-// HBM speed (measured 1.7 TB/s over a whole 8B decode step, profiles/r02_decode_*.json): the step is pure weight
-// bandwidth, so this kernel does the minimum — every weight byte is loaded exactly once with 16-byte coalesced vectors,
+// With <= 8 rows the 128-row wgmma tile wastes > 93 % of the tensor pipe, and the step is pure weight bandwidth, so this
+// kernel does the minimum — every weight byte is loaded exactly once with 16-byte coalesced vectors,
 // 16 loads in flight per lane, and multiplied on the FMA pipe against the activation rows held in shared memory.
 //   block = 8 warps, one warp = 2 output columns; K is walked in chunks of 2048 (x chunk: M x 4 KB of smem);
 //   fp32 accumulation, one shuffle tree per (row, column) at the end.

@@ -168,11 +168,11 @@ int preprocess_launch(const uint8_t* img, int H, int W, int R, const int* pad_rg
     return set_error(CB_ERR_CUDA, "preprocess: coefficient upload failed: %s", cudaGetErrorString(cudaGetLastError()));
   const int threads = 256;
   long long nb = ((long long)S * R + threads - 1) / threads;
-  resample_h_kernel<<<(unsigned)std::min<long long>(nb, 148LL * 32), threads, 0, st>>>(
+  resample_h_kernel<<<(unsigned)std::min<long long>(nb, device_sm_count() * 32LL), threads, 0, st>>>(
       img, H, W, S, off_y, off_x, R, d_bounds, d_kk, ksize, pad_rgb[0], pad_rgb[1], pad_rgb[2], tmp);
   CB_CUDA_LAUNCH_CHECK("resample_h");
   nb = ((long long)R * R + threads - 1) / threads;
-  resample_v_norm_kernel<<<(unsigned)std::min<long long>(nb, 148LL * 32), threads, 0, st>>>(
+  resample_v_norm_kernel<<<(unsigned)std::min<long long>(nb, device_sm_count() * 32LL), threads, 0, st>>>(
       tmp, R, d_bounds, d_kk, ksize, mean[0], mean[1], mean[2], 1.0f / std_[0], 1.0f / std_[1], 1.0f / std_[2],
       (bf16*)out, out_u8);
   CB_CUDA_LAUNCH_CHECK("resample_v_norm");

@@ -14,10 +14,9 @@ buffers for bf16 gradients, fp32 master weights and fp32 Adam moments:
   * the optimizer is a fused AdamW kernel over contiguous SEGMENTS of equal hyper-parameters (the reference's parameter
     groups, cambrian_trainer.py:242-381: `mm_projector_lr` / `mm_vision_sampler_lr` group learning rates, no weight decay
     for norm and bias parameters) on a side stream.  `background_optimizer=True` launches it as ONE small block per SM so it
-    co-resides with persistent GEMM CTAs; measured on the power-capped B200 that is a net LOSS (the chip is at its 1 kW cap
-    either way, the HBM-bound update then crawls at 1.7 TB/s for 135 ms and drags the GEMMs it shares HBM with from 0.795 to
-    0.739 of peak: 8.24 vs 8.68 samples/s, profiles/r02_bench_variants.md), so the default is the full-occupancy launch
-    (4.9 TB/s, 47 ms) placed where it overlaps the frozen towers of the next step;
+    co-resides with GEMM CTAs; the default is the full-occupancy launch placed where it overlaps the frozen towers of the
+    next step, because a slow HBM-bound update that shares HBM with the GEMMs for its whole duration costs them more than
+    it saves (measured on an earlier GPU generation; not re-measured on H100);
   * gradient clipping (`max_grad_norm`, HF Trainer's default 1.0 is active in every reference script): per-bucket sums of
     squares are taken as the buckets arrive, the clip coefficient stays on the device (no host sync) and is applied inside
     AdamW.  Because no update may start before the global norm is known, with clipping the updates run after backward, in

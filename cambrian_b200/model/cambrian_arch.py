@@ -1,4 +1,4 @@
-"""Multimodal glue — B200-native mirror of the reference's `cambrian/model/cambrian_arch.py`.
+"""Multimodal glue — H100-native mirror of the reference's `cambrian/model/cambrian_arch.py`.
 
 `CambrianMetaModel` builds the same sub-modules with the same attribute / state-dict names (mm_projector,
 mm_projector_aux_{i}, vision_sampler_{g}, vision_sampler_layers, vision_query, image_newline; cambrian_arch.py:35-87,
@@ -177,7 +177,7 @@ class CambrianMetaForCausalLM(ABC):
 
     def encode_images(self, image_aux_list):
         """cambrian_arch.py:332-338.  The towers are independent of each other (and frozen in every released recipe), so
-        each runs on its own CUDA stream: most ViT GEMMs are a wave and a bit on 148 SMs (M = B * 577 rows -> 152 tiles),
+        each runs on its own CUDA stream: most ViT GEMMs are a wave and a bit on 132 SMs (M = B * 577 rows -> ~150 tiles),
         and with one-CTA-per-tile grids the idle SMs of one tower's last wave take tiles of another tower's kernel instead
         of waiting (CB_TOWER_STREAMS=0 runs them back to back on the current stream)."""
         towers = self.get_model().get_vision_tower_aux_list()

@@ -1,4 +1,4 @@
-"""CambrianLlamaForCausalLM — B200-native mirror of the reference's `cambrian/model/language_model/cambrian_llama.py`.
+"""CambrianLlamaForCausalLM — H100-native mirror of the reference's `cambrian/model/language_model/cambrian_llama.py`.
 
 Same public surface (SURVEY.md §8b): `CambrianConfig` (model_type "cambrian_llama"), `CambrianLlamaModel`,
 `CambrianLlamaForCausalLM.forward(input_ids, attention_mask, position_ids, past_key_values, inputs_embeds, labels,
@@ -6,7 +6,7 @@ use_cache, output_attentions, output_hidden_states, images, image_aux_attention_
 cache_position)`, `generate(inputs, images, image_sizes, **kw)`, `get_model()`, HF auto-class registration, and the
 HF LLaMA state-dict keys (`model.layers.{i}.self_attn.q_proj.weight`, ...), so released checkpoints load unchanged.
 
-Every decoder layer runs as one `DecoderLayerFn` (RMSNorm -> fused QKV tcgen05 GEMM -> RoPE -> tcgen05 flash attention
+Every decoder layer runs as one `DecoderLayerFn` (RMSNorm -> fused QKV wgmma GEMM -> RoPE -> wgmma flash attention
 -> o-proj GEMM + residual -> RMSNorm -> fused gate/up GEMM -> SwiGLU -> down GEMM + residual), with the SVA layers
 re-inserted on the image span after decoder layers start + k*stride exactly as cambrian_llama.py:168-207 does.
 q/k/v (and gate/up) keep their HF parameter names but share one contiguous storage so each pair/triple is one GEMM.
@@ -553,8 +553,8 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
 
     def _generate_graphed(self, args, cache, h_last, next_pos, S0, max_new, check_stop):
         """Greedy decoding with ONE CUDA graph per generate() call: a decode step is ~290 kernel launches whose device time
-        (weight streaming, a few ms) is far below the cost of enqueueing them one by one from Python (8.3 ms / token for the
-        8B shape, profiles/r02_decode_b1_eager_loop.json), so the step is captured once — static shapes: token / position /
+        (weight streaming, a few ms) is far below the cost of enqueueing them one by one from Python, so the step is captured
+        once — static shapes: token / position /
         cache-slot / validity mask live in device buffers that the captured kernels advance themselves — and replayed per
         token.  EOS / stopping criteria are evaluated between replays on the host exactly as in the eager loop."""
         from ...generation import should_stop

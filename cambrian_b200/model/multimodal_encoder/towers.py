@@ -1,4 +1,4 @@
-"""The four Cambrian-1 vision towers, forward-only on hand-written sm_100a kernels.
+"""The four Cambrian-1 vision towers, forward-only on hand-written sm_90a kernels.
 
 Mirrors the reference wrappers (cambrian/model/multimodal_encoder/{base,clip,siglip,dino,clip_convnext}_encoder.py):
 same class names, name parsing (`-res{N}`, `-interp{N}`), properties and `forward(images) -> [B, N, C]`, and the

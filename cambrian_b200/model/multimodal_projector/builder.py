@@ -1,6 +1,6 @@
 """`build_vision_projector` — mirror of cambrian/model/multimodal_projector/builder.py:54-78 for the projector types the
 hot path uses (`linear`, `mlp{N}x_gelu`, `identity`).  Returns nn.Sequential modules with the reference's state-dict
-keys (0.weight, 0.bias, 2.weight, ...), whose Linear / GELU children run on the sm_100a GEMM / activation kernels."""
+keys (0.weight, 0.bias, 2.weight, ...), whose Linear / GELU children run on the sm_90a GEMM / activation kernels."""
 from __future__ import annotations
 
 import re

@@ -1,10 +1,10 @@
-"""Spatial Vision Aggregator — B200-native mirror of the reference's `cambrian/model/vision_sampler.py`.
+"""Spatial Vision Aggregator — H100-native mirror of the reference's `cambrian/model/vision_sampler.py`.
 
 Same class names, constructor signatures, attribute / state-dict key names and call conventions as the reference
 (`VisionTokenSampler` vision_sampler.py:407-419, `VisionCrossAttentionLayer` :248-327, `MultiKVCrossAttention`
 :155-234, `MLP` :237-245), so released checkpoints load unchanged and `cambrian_arch` / `cambrian_llama` call sites work
-as they are.  The arithmetic runs in `cambrian_b200.autograd.SVALayerFn` on the hand-written sm_100a kernels
-(tcgen05 GEMMs for the LayerNorm+Linear projections, the fused window-attention kernel for the softmax).
+as they are.  The arithmetic runs in `cambrian_b200.autograd.SVALayerFn` on the hand-written sm_90a kernels
+(wgmma GEMMs for the LayerNorm+Linear projections, the fused window-attention kernel for the softmax).
 
 Both layer types are implemented: `joint` (`VisionCrossAttentionLayer`, the one every released model and every reference
 caller uses — one hand-scheduled `SVALayerFn` block) and `sep` (`VisionAggregationLayer` :330-405 with `CrossAttention`
@@ -55,7 +55,7 @@ class VisionCrossAttentionLayer(nn.Module):
         super().__init__()
         num_heads = 16
         if hidden_dim != 1024 or any(d != hidden_dim for d in kv_dim_list):
-            raise NotImplementedError("the sm_100a SVA kernels are specialised for vision_hidden_size = 1024 (16 x 64)")
+            raise NotImplementedError("the SVA kernels are specialised for vision_hidden_size = 1024 (16 x 64)")
         self.num_of_kvs = len(kv_dim_list)
         self.q_dim = q_dim
         self.proj_context = nn.Linear(context_dim, hidden_dim, bias=False)
@@ -158,7 +158,7 @@ class VisionAggregationLayer(nn.Module):
         super().__init__()
         num_heads = 16
         if hidden_dim != 1024 or any(d != hidden_dim for d in kv_dim_list):
-            raise NotImplementedError("the sm_100a SVA kernels are specialised for vision_hidden_size = 1024 (16 x 64)")
+            raise NotImplementedError("the SVA kernels are specialised for vision_hidden_size = 1024 (16 x 64)")
         self.num_of_kvs = len(kv_dim_list)
         if self.num_of_kvs > NarrowLinearFn.PAD:
             raise NotImplementedError(f"at most {NarrowLinearFn.PAD} towers")

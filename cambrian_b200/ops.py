@@ -1,6 +1,6 @@
 """Raw (non-autograd) Python wrappers over the C ABI: one function per entry point of
 include/cambrian_b200.h.  Tensors are torch CUDA tensors used purely as device buffers; every call
-launches the hand-written sm_100a kernel on the current torch stream.  No fallbacks."""
+launches the hand-written sm_90a kernel on the current torch stream.  No fallbacks."""
 from __future__ import annotations
 
 import ctypes
@@ -109,9 +109,8 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
     N, Kb = (bc, br) if b_mn else (br, bc)
     if K != Kb or ba != bb:
         raise ValueError(f"gemm: shape mismatch a={tuple(a.shape)} b={tuple(b.shape)} a_mn={a_mn} b_mn={b_mn}")
-    # decode step: weight streaming.  The CUDA-core GEMV is FMA-bound at 6-8 rows (2.0-2.6 TB/s at M = 8): for wide outputs
-    # the 128-row tcgen05 tile streams the weights faster there (measured, profiles/r02_probe_gemv.log: N = 28672: 61 vs
-    # 97 us, N = 128256: 257 vs 396 us at M = 8; N <= 6144: GEMV wins at every M), so those keep the tensor-core kernel.
+    # decode step: weight streaming.  The CUDA-core GEMV is FMA-bound at 6-8 rows, so wide outputs (N >= 16384) at
+    # those row counts keep the tensor-core kernel (a threshold carried over from an earlier GPU; not re-measured on H100).
     if (_GEMV and M <= 8 and not (M >= 6 and N >= 16384) and not batched and not a_mn and not b_mn
             and act in (None, "none") and colscale is None
             and not accumulate and alpha == 1.0 and force_bn == 0 and K % 8 == 0 and lda % 8 == 0 and ldb % 8 == 0
@@ -158,11 +157,6 @@ def gemv(x: torch.Tensor, w: torch.Tensor, bias=None, residual=None, out=None, o
                                    ptr(residual), residual.stride(0) if residual is not None else 0,
                                    int(out.dtype == torch.float32), stream()), "cb_gemv_bf16")
     return out
-
-
-def gemm_set_dynamic_scheduling(on: bool) -> bool:
-    """Cluster-Launch-Control tile scheduling for the persistent GEMMs (default on); returns the previous setting."""
-    return bool(_lib.load().cb_gemm_set_dynamic_scheduling(int(on)))
 
 
 def linear(x: torch.Tensor, weight: torch.Tensor, bias=None, **kw) -> torch.Tensor:
@@ -325,7 +319,7 @@ def attn_bwd(q, k, v, o, do, lse, *, causal: bool, kmask=None, scale: float | No
         scale = hd ** -0.5
     dev = q.device
     delta = torch.empty((B, nh, Sq), dtype=torch.float32, device=dev)
-    dq_acc = torch.zeros((B, Sq, nh, hd), dtype=torch.float32, device=dev)
+    dq_acc = torch.empty((B, Sq, nh, hd), dtype=torch.float32, device=dev)   # every element written once
     dk = dk if dk is not None else torch.empty((B, Skv, nkv, hd), dtype=torch.bfloat16, device=dev)
     dv = dv if dv is not None else torch.empty((B, Skv, nkv, hd), dtype=torch.bfloat16, device=dev)
     qb, qs = _bshd_strides(q, hd)
@@ -700,18 +694,18 @@ def gemm_swiglu(x2d, w_gu, gu_out=None, act_out=None):
     return gu, act
 
 
-# CB_FUSED_SWIGLU=0 falls back to GEMM + stand-alone SwiGLU kernel (A/B switch used for profiles/, both are CUDA paths)
+# CB_FUSED_SWIGLU=0 runs GEMM + the stand-alone SwiGLU kernel instead (an A/B switch; both are CUDA paths)
 _FUSED_SWIGLU = os.environ.get("CB_FUSED_SWIGLU", "1") != "0"
 
 
 def mlp_gate_up(h2d, w_gu):
-    """gate/up projection + SwiGLU: the fused CTA-pair kernel when the problem fills the SM pairs for >= 3 waves (the
-    same rule cb_gemm_bf16 uses to pick that kernel) and F % 128 == 0, otherwise GEMM followed by the SwiGLU kernel."""
+    """gate/up projection + SwiGLU: the fused kernel (128-row x 64-feature tiles) when the problem fills the SMs for >= 3
+    waves and F % 128 == 0, otherwise GEMM (whose tile width adapts to small problems) followed by the SwiGLU kernel."""
     M = h2d.shape[0]
     F2 = w_gu.shape[0]
     I = F2 // 2
-    pairs = max(_lib.load().cb_sm_count() // 2, 1)
-    if (_FUSED_SWIGLU and F2 % 256 == 0 and ((M + 255) // 256) * (F2 // 256) >= 3 * pairs and h2d.is_contiguous()
+    sms = max(_lib.load().cb_sm_count(), 1)
+    if (_FUSED_SWIGLU and F2 % 256 == 0 and ((M + 127) // 128) * (F2 // 128) >= 3 * sms and h2d.is_contiguous()
             and w_gu.is_contiguous()):
         return gemm_swiglu(h2d, w_gu)
     gu = gemm(h2d, w_gu)

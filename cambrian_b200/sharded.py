@@ -1,7 +1,7 @@
-"""ZeRO-3 style parameter sharding for inference (BASELINE config 5: Cambrian-34B `generate` on 8 x B200).
+"""ZeRO-3 style parameter sharding for inference (BASELINE config 5: Cambrian-34B `generate` on 8 GPUs).
 
 The reference reaches this configuration through DeepSpeed ZeRO-3 (`scripts/zero3.json:16-27`) / `device_map="auto"`
-(model/builder.py:29-33).  B200-native design (SURVEY.md §8e): one process per GPU, the decoder layers — 97 % of the
+(model/builder.py:29-33).  Design (SURVEY.md §8e): one process per GPU, the decoder layers — 97 % of the
 parameters — are flattened per layer and every rank keeps 1/world of each layer; a layer's full weights exist only in
 one of two staging buffers, all-gathered over NCCL/NVLink one layer AHEAD of the layer being computed, so the gather of
 layer i+1 overlaps the GEMMs of layer i.  The gather wraps around (the last layer prefetches layer 0), which keeps the

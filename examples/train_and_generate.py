@@ -1,4 +1,4 @@
-"""Minimal end-to-end use of the drop-in modules on one B200 (random-init, synthetic batch; mirrors what
+"""Minimal end-to-end use of the drop-in modules on one H100 (random-init, synthetic batch; mirrors what
 tests/test_modules_gpu.py exercises — the model / collator / engine calls are the ones a training loop makes).
 
     python -m cambrian_b200.build          # once

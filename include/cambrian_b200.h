@@ -1,4 +1,4 @@
-/* cambrian_b200 — C ABI of the B200-native Cambrian-1 hot-path kernels (libcambrian_b200.so).
+/* cambrian_b200 — C ABI of the H100-native (sm_90a) Cambrian-1 hot-path kernels (libcambrian_b200.so).
  *
  * The reference (cambrian-mllm/cambrian) has NO FFI / plugin layer: its hot path is Python
  * nn.Modules that dispatch torch ops (SURVEY.md §2a, §8b).  This header therefore declares the
@@ -42,7 +42,7 @@ int cb_sm_count(void);
 /* number of kernels this library has launched in this process (bench.py reports the per-step delta as gpu_launches) */
 int64_t cb_launch_count(void);
 
-/* ---- dense contraction: tcgen05 + TMA persistent GEMM --------------------------------------
+/* ---- dense contraction: wgmma + TMA GEMM ----------------------------------------------------
  * C[b] (M x N row-major, ldc)  (+)=  epi( alpha * opA(A[b]) (M x K) * opB(B[b]) (K x N) )
  *   a_mn = 0: A is [M, K] with K contiguous (lda);  a_mn = 1: A is [K, M] with M contiguous
  *   b_mn = 0: B is [N, K] with K contiguous (ldb) — the nn.Linear weight layout;  b_mn = 1: [K, N]
@@ -97,7 +97,7 @@ int cb_rmsnorm_bwd(const void* dy, const void* x, const void* gamma, const float
                    void* stream);
 int64_t cb_norm_bwd_workspace_floats(int64_t rows, int C);
 
-/* ---- softmax attention: tcgen05 flash attention ------------------------------------------------
+/* ---- softmax attention: wgmma flash attention --------------------------------------------------
  * q/k/v/o element (b, s, head, d) lives at base + b*bs + s*ss + head*hd + d (element strides), so the packed
  * QKV GEMM output is consumed in place.  nh % nkv == 0 (GQA).  kmask [B, Skv] bool (1 byte, 1 = attend) or NULL.
  * causal: key k visible to query i iff k <= i + (Skv - Sq).  lse [B, nh, Sq] fp32 (log2 domain) may be NULL.
@@ -107,8 +107,9 @@ int64_t cb_norm_bwd_workspace_floats(int64_t rows, int C);
 int cb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, const void* kmask, int B, int nh,
                 int nkv, int Sq, int Skv, int hd, int64_t q_bs, int64_t q_ss, int64_t k_bs, int64_t k_ss,
                 int64_t v_bs, int64_t v_ss, int64_t o_bs, int64_t o_ss, float scale, int causal, void* stream);
-/* delta [B, nh, Sq] fp32 scratch; dq_acc [B, Sq, nh, hd] fp32 ZERO-INITIALISED by the caller, receives the
- * unscaled sum dS K (multiply by `scale` when converting, cb_f32_to_bf16); dk/dv written (bf16, strided). */
+/* delta [B, nh, Sq] fp32 scratch; dq_acc [B, Sq, nh, hd] fp32 receives the unscaled sum dS K (multiply by `scale` when
+ * converting, cb_f32_to_bf16); dk/dv written (bf16, strided).  Every output element has one writer (no atomics), so the
+ * results are bit-identical from run to run. */
 int cb_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                 float* delta, float* dq_acc, void* dk, void* dv, const void* kmask, int B, int nh, int nkv, int Sq,
                 int Skv, int hd, int64_t q_bs, int64_t q_ss, int64_t k_bs, int64_t k_ss, int64_t v_bs, int64_t v_ss,
@@ -186,7 +187,7 @@ int cb_embed_splice_ragged(void* out, const void* embed, const void* img, const 
                            int64_t rows, int H, void* stream);
 /* LLaMA MLP first half in one launch (HF LlamaMLP, reached from cambrian_llama.py:142-166): W = [gate_proj; up_proj]
  * [2F, K]; gu_out [M, 2F] = A W^T (bf16 pre-activations, saved for backward), act_out [M, F] = silu(gate) * up.
- * F % 128 == 0.  CTA-pair tcgen05 kernel whose tile pairs 128 gate columns with the matching 128 up columns. */
+ * F % 128 == 0.  wgmma GEMM whose tile pairs 64 gate columns with the matching 64 up columns. */
 int cb_gemm_swiglu_bf16(const void* A, const void* W, void* gu_out, void* act_out, int M, int F, int K, int64_t lda,
                         int64_t ldw, int64_t ld_gu, int64_t ld_act, void* stream);
 /* Image preprocessing on the GPU (SURVEY.md 8f rank 4) — replaces, per tower, the host chain of `process_images`
@@ -230,10 +231,6 @@ int cb_gemv_bf16(const void* x, const void* w, void* y, int M, int N, int K, int
  * call.  nbytes % (16 * world) == 0.  Every rank must issue the same calls in the same order. */
 int cb_allreduce_symm_bf16(uint64_t multicast_base, const uint64_t* buffer_ptrs, const uint64_t* signal_pad_ptrs,
                            int64_t offset_bytes, int64_t nbytes, int rank, int world, uint32_t epoch, int ctas, void* stream);
-/* GEMM tile scheduling: 1 (default; env CB_GEMM_CLC=0 to start with 0) = one CTA / CTA pair per tile in the grid, tiles
- * handed out by Cluster Launch Control so the GEMM tolerates SMs held by collectives / the background optimizer;
- * 0 = static persistent walk.  Returns the previous setting.  Results are bit-identical either way. */
-int cb_gemm_set_dynamic_scheduling(int on);
 /* acc[0] += sum of squares of n bf16 values (deterministic two-stage reduction; workspace >= grid floats, 4096 suffices) */
 int cb_sumsq_bf16(const void* g, int64_t n, float* acc, float* workspace, int64_t workspace_floats, int background,
                   void* stream);

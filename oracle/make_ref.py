@@ -4,10 +4,9 @@
 
 The reference is pure Python; the one file of its hot path that needs nothing but torch is
 `cambrian/model/vision_sampler.py` (VisionTokenSampler, vision_sampler.py:407-419).  It is copied VERBATIM, byte for
-byte, from where it lies under /root/reference into oracle/_ref/ — a git-ignored OUTPUT directory that travels to the GPU
-box with the snapshot like a built .so does (it is not listed in .gpurunignore) — so that the CPU arm of bench.py
-(oracle/cpu_arm.py) can time the reference's real module on the GPU box's host cores, where /root/reference does not
-exist.  Nothing under oracle/_ref/ is committed, imported by the product, or edited.
+byte, from where it lies under /root/reference into oracle/_ref/ — a git-ignored build OUTPUT, like the built .so — so
+that the CPU arm of bench.py (oracle/cpu_arm.py) can time the reference's real module on machines where the reference
+tree does not exist.  Nothing under oracle/_ref/ is committed, imported by the product, or edited.
 """
 from __future__ import annotations
 

@@ -1,8 +1,8 @@
 """TEST INFRASTRUCTURE ONLY — import shim for the *unmodified* reference modules under /root/reference.
 
-Only used in the build container (the GPU box has no /root/reference) to (a) pin the CPU oracle in
-`oracle/*.py` against the reference's own code and (b) generate the committed golden fixtures in
-`tests/golden/` (generator: tests/golden/make_golden.py).  Nothing in the product imports this.
+Only used where the reference tree exists, to generate the committed golden fixtures in `tests/golden/` that pin the CPU
+oracle in `oracle/*.py` against the reference's own code (generator: tests/golden/make_golden.py).  Nothing in the
+product or the test suite imports this.
 
 The reference package cannot be imported normally (SURVEY.md §8c): `cambrian/__init__.py` eagerly imports
 every encoder, which needs timm / open_clip / diffusers / ezcolorlog / torch_xla.  Recipe: stub those
@@ -51,7 +51,7 @@ def install() -> None:
     if _installed:
         return
     if not available():
-        raise RuntimeError("/root/reference is not present (GPU box?) — the shim only works in the build container")
+        raise RuntimeError("/root/reference is not present — the shim needs the reference tree")
     import transformers  # noqa: F401  (must be imported before the stubs shadow anything it probes)
     sys.meta_path.insert(0, _StubFinder())
     for pkg in ("cambrian", "cambrian.model", "cambrian.model.multimodal_encoder",

@@ -1,7 +1,7 @@
-"""Generates the committed golden fixtures from the UNMODIFIED reference modules (run in the build container only:
-/root/reference does not exist on the GPU box).
+"""Generates the committed golden fixtures from the UNMODIFIED reference modules (run where the reference tree exists;
+nothing else in the repository needs it).
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py            (--only-pins: just the pin_*.npz fixtures)
 
 Weights are not stored: every parameter is regenerated from numpy's PCG64 stream (stable across numpy versions) by
 `seeded_fill`, in state-dict order, so the fixtures stay a few hundred KB.  Each .npz holds the seeded inputs and the
@@ -14,6 +14,10 @@ reference's outputs for:
                    rearrange_vision_tower_features_inference (cambrian_arch.py:203-330) and the whole
                    prepare_inputs_labels_for_multimodal dynamic path (:340-451, :493-609) run on a stub model that
                    holds reference modules (VisionTokenSampler, nn.Sequential projectors) under the reference's names
+  pin_*.npz        what the reference modules compute in the oracle pins of tests/test_oracle_pin.py and
+                   tests/test_host_logic_cpu.py: sep sampler output + sampled gradients, config 1 at full size, two query
+                   groups through prepare_inputs_labels_for_multimodal, the mlp2x_gelu projector, state-dict layouts,
+                   unmask_attention_mask / unpad_image on random sizes
 """
 from __future__ import annotations
 
@@ -203,9 +207,206 @@ def make_sep(vs):
         print(name, tuple(out.shape), float(out.abs().mean()))
 
 
+# ------------------------------------------------------------------------------------------------------------------
+# pins of the oracle against the reference modules: what the reference computed, stored so the comparison needs no
+# reference tree (tests/test_oracle_pin.py, tests/test_host_logic_cpu.py)
+# ------------------------------------------------------------------------------------------------------------------
+SEP_LIVE_CASES = [([1, 2, 1], 256, 2), ([3], 512, 1), ([1], 1024, 1)]
+GRAD_SAMPLES = 32
+OUT_SAMPLES = 256
+
+
+def sd_layout(sd):
+    """parameter names / shapes in state-dict order: enough to regenerate seeded_fill weights without the module"""
+    return dict(sd_keys=np.array(list(sd.keys())), sd_shapes=np.array([",".join(map(str, v.shape)) for v in sd.values()]))
+
+
+def sd_from_layout(z, seed):
+    shapes = {str(k): tuple(int(x) for x in str(sh).split(",") if x) for k, sh in zip(z["sd_keys"], z["sd_shapes"])}
+    return seeded_fill({k: torch.empty(v) for k, v in shapes.items()}, seed)
+
+
+def grad_sample_index(numels, seed=74):
+    """fixed sample of GRAD_SAMPLES flat indices per gradient tensor"""
+    rng = np.random.default_rng(seed)
+    return [rng.integers(0, n, size=min(GRAD_SAMPLES, n)) for n in numels]
+
+
+def flat_sample(t, k=OUT_SAMPLES, seed=75):
+    """a fixed seeded sample of k elements of t (all of them if t is smaller): keeps the pin fixtures a few KB"""
+    n = t.numel()
+    if n <= k:
+        return t.reshape(-1)
+    idx = np.random.default_rng(seed).integers(0, n, size=k)
+    return t.reshape(-1)[torch.from_numpy(idx)]
+
+
+def sep_live_dy(shape):
+    return torch.from_numpy(np.random.default_rng(73).standard_normal(tuple(shape)).astype(np.float32))
+
+
+def config1_inputs(rs, seed):
+    from oracle import cambrian_oracle as O
+    g = torch.Generator().manual_seed(seed)
+    feats = [torch.randn(1, (24 * r) ** 2, 1024, generator=g) for r in rs]
+    query = (torch.randn(1, 1024, generator=g) / 32).view(1, 1, 1, -1).expand(1, 576, -1, -1).flatten(0, 1)
+    ctx = feats[0].mean(1).view(1, 1, 1, -1).expand(-1, 576, 1, -1).flatten(0, 1)
+    fw = [O.window_rearrange(f, 24) for f in feats]
+    masks = [torch.rand(576, r * r, generator=g) > 0.2 for r in rs]
+    for mk in masks:
+        mk[mk.sum(1) == 0] = True
+    return query, ctx, fw, masks
+
+
+TWO_GROUPS = dict(H=64, q=4, sides=[4, 8], dims=[48, 40], B=2, seed=91)
+
+
+def two_groups_inputs():
+    c = TWO_GROUPS
+    g = torch.Generator().manual_seed(c["seed"] + 1)
+    q, B = c["q"], c["B"]
+    feats = [torch.randn(B, s * s, d, generator=g) for s, d in zip(c["sides"], c["dims"])]
+    masks = [torch.ones(B * q * q, (s // q) ** 2, dtype=torch.bool) for s in c["sides"]]
+    masks[1][::5, 1] = False
+    span = q * (q + 1)
+    ids = torch.randint(3, 100, (B, 5 + span + 6), generator=g)
+    ids[:, 5] = -200
+    ids[:, 6:5 + span] = 0
+    return feats, masks, ids
+
+
+def projector_input():
+    return torch.from_numpy(np.random.default_rng(96).standard_normal((3, 7, 96)).astype(np.float32))
+
+
+def unpad_cases():
+    rng = np.random.default_rng(5)
+    cases = []
+    for _ in range(300):
+        w, h = int(rng.integers(16, 4000)), int(rng.integers(16, 4000))
+        cases.append((w, h, int(rng.choice([16, 24, 27, 48, 96]))))
+    return cases
+
+
+def make_pins(vs, arch):
+    import torch.nn as nn
+    from oracle import ref_shim
+    # layer_type="sep": output and every gradient of the reference module (gradients as a fixed sample + their norms)
+    recs = {}
+    for i, (rs, q_dim, layers) in enumerate(SEP_LIVE_CASES):
+        m = vs.VisionTokenSampler(q_dim, 1024, [1024] * len(rs), rs, 1024, layers, layer_type="sep")
+        sd = seeded_fill(m, 71)
+        m.load_state_dict(sd)
+        queries, ctx, feats, masks = seeded_inputs(72, 10, q_dim, rs)
+        queries.requires_grad_()
+        ref = m(queries, ctx, *feats, *masks)
+        params = list(m.named_parameters())
+        grads = torch.autograd.grad(ref, [queries] + [p for _, p in params], sep_live_dy(ref.shape))
+        idx = grad_sample_index([g.numel() for g in grads])
+        recs.update({f"c{i}_" + k: v for k, v in sd_layout(sd).items()})
+        recs[f"c{i}_names"] = np.array([k for k, _ in params])
+        recs[f"c{i}_out"] = flat_sample(ref.detach()).numpy()
+        recs[f"c{i}_outsum"] = ref.detach().sum(-1).numpy()
+        recs[f"c{i}_gsample"] = np.concatenate([g.reshape(-1)[torch.from_numpy(ix)].numpy() for g, ix in zip(grads, idx)])
+        recs[f"c{i}_gnorm"] = np.array([g.double().norm().item() for g in grads])
+    np.savez_compressed(os.path.join(HERE, "pin_sep_fwd_bwd.npz"), **recs)
+    # BASELINE config 1 at full size, random masks: a fixed sample of the output + all row sums
+    recs = {}
+    for j, rs in enumerate(([1, 1, 1, 1], [1, 1, 1, 4])):
+        m = vs.VisionTokenSampler(1024, 1024, [1024] * 4, rs, 1024, 3).eval()
+        sd = seeded_fill(m, 81 + j)
+        m.load_state_dict(sd)
+        query, ctx, fw, masks = config1_inputs(rs, 82 + j)
+        with torch.no_grad():
+            ref = m(query, ctx, *fw, *masks)[:, 0]
+        recs.update({f"r{j}_" + k: v for k, v in sd_layout(sd).items()})
+        recs[f"r{j}_sample"] = flat_sample(ref, 512).numpy()
+        recs[f"r{j}_rowsum"] = ref.sum(1).numpy()
+    np.savez_compressed(os.path.join(HERE, "pin_config1.npz"), **recs)
+    # two query groups through the reference's static-branch prepare_inputs_labels_for_multimodal
+    c = TWO_GROUPS
+    H, q, sides, dims = c["H"], c["q"], c["sides"], c["dims"]
+
+    class Inner(nn.Module):
+        def __init__(self):
+            super().__init__()
+            for i, d in enumerate(dims):
+                setattr(self, f"mm_projector_aux_{i}", nn.Sequential(nn.Linear(d, 1024), nn.GELU(), nn.Linear(1024, 1024),
+                                                                     nn.LayerNorm(1024)))
+            self.vision_sampler_0 = vs.VisionTokenSampler(1024, 1024, [1024, 1024], [s // 4 for s in sides], 1024, 2)
+            self.vision_sampler_1 = vs.VisionTokenSampler(1024, 1024, [1024, 1024], [s // 2 for s in sides], 1024, 2)
+            self.mm_projector = nn.Sequential(nn.Linear(2048, H), nn.GELU(), nn.Linear(H, H))
+            self.embed_tokens = nn.Embedding(100, H)
+            self.vision_query = nn.Parameter(torch.zeros(2, 1024))
+            self.image_newline = nn.Parameter(torch.zeros(H))
+            self.config = type("C", (), dict(image_token_len=q * q, query_num_list=[q * q, 4], mm_projector_type="sva"))()
+
+        def get_vision_tower_aux_list(self):
+            return [lambda x: x for _ in dims]
+
+    class Top(nn.Module, arch.CambrianMetaForCausalLM):
+        def __init__(self):
+            nn.Module.__init__(self)
+            self.model = Inner()
+            self.config = self.model.config
+            self.device = torch.device("cpu")
+
+        def get_model(self):
+            return self.model
+
+    top = Top().eval()
+    sd = seeded_fill(top.model, c["seed"])
+    top.model.load_state_dict(sd)
+    feats, masks, ids = two_groups_inputs()
+    flag = arch.IS_XLA_AVAILABLE
+    arch.IS_XLA_AVAILABLE = True
+    try:
+        with torch.no_grad():
+            out = top.prepare_inputs_labels_for_multimodal(ids, None, None, None, None, feats, masks, None)
+    finally:
+        arch.IS_XLA_AVAILABLE = flag
+    recs = dict(sd_layout(sd), emb=flat_sample(out[4]).numpy(), embsum=out[4].sum(-1).numpy())
+    for i, f in enumerate(out[6]):          # window-rearranged aux features handed to the in-LLM SVA layers (sampled)
+        recs[f"feat_w{i}"] = flat_sample(f).numpy()
+    np.savez_compressed(os.path.join(HERE, "pin_two_groups.npz"), **recs)
+    # mlp2x_gelu projector
+    pb = ref_shim.ref_module("cambrian.model.multimodal_projector.builder")
+    from types import SimpleNamespace
+    proj = pb.build_vision_projector(SimpleNamespace(mm_projector_type="mlp2x_gelu", mm_hidden_size=96, hidden_size=64)).eval()
+    sd = seeded_fill(proj, 95)
+    proj.load_state_dict(sd)
+    with torch.no_grad():
+        y = proj(projector_input())
+    np.savez_compressed(os.path.join(HERE, "pin_projector.npz"), **sd_layout(sd), out=flat_sample(y).numpy())
+    # state-dict layouts of the reference samplers
+    recs = {}
+    for i, args in enumerate([(1024, 1024, [1024] * 4, [1, 1, 1, 1], 1024, 3), (256, 1024, [1024] * 3, [1, 2, 3], 1024, 1)]):
+        recs[f"keys{i}"] = np.array(list(vs.VisionTokenSampler(*args).state_dict()))
+    recs.update({"sep_" + k: v for k, v in sd_layout(vs.VisionTokenSampler(256, 1024, [1024] * 3, [2, 1, 3], 1024, 2,
+                                                                          layer_type="sep").state_dict()).items()})
+    np.savez_compressed(os.path.join(HERE, "pin_state_dicts.npz"), **recs)
+    # unmask_attention_mask / unpad_image on random image sizes: the mask (packed bits) and the crop unpad_image keeps
+    masks, crops = [], []
+    for (w, h, side) in unpad_cases():
+        masks.append(np.packbits(arch.unmask_attention_mask(torch.ones(1, side, side, dtype=torch.bool), (w, h)).numpy()))
+        t = torch.arange(side * side).view(1, side, side, 1)
+        u = arch.unpad_image(t, (w, h))
+        if 0 in u.shape:
+            crops.append((-1, -1, -1, -1))
+        else:
+            v = u[0, :, :, 0]
+            crops.append((int(v[0, 0]) // side, int(v[-1, 0]) // side + 1, int(v[0, 0]) % side, int(v[0, -1]) % side + 1))
+    np.savez_compressed(os.path.join(HERE, "pin_unpad.npz"), masks=np.concatenate(masks), mask_lens=np.array([len(m) for m in masks]),
+                        crops=np.array(crops))
+    print("pins written")
+
+
 def main():
     from oracle import ref_shim
     vs = ref_shim.ref_module("cambrian.model.vision_sampler")
+    if "--only-pins" in sys.argv:
+        make_pins(vs, ref_shim.ref_module("cambrian.model.cambrian_arch"))
+        return
     if "--only-sep" in sys.argv:
         make_sep(vs)
         return
@@ -278,6 +479,7 @@ def main():
     np.savez_compressed(os.path.join(HERE, "collator.npz"), **recs)
     print("collator", len(recs))
     make_dynamic(arch, vs)
+    make_pins(vs, arch)
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""Kernel-level GPU parity tests, called through the C ABI (ctypes): every case compares one hand-written sm_100a kernel
+"""Kernel-level GPU parity tests, called through the C ABI (ctypes): every case compares one hand-written sm_90a kernel
 with a plain PyTorch fp32 reference of the same op on seeded inputs.  The case tables live in tools/probe1.py /
 tools/probe2.py (they print one line per case, which doubles as the profiling log); a case that misses its tolerance
 prints FAIL.  Tolerances: GEMM with fp32 output 2e-5 relative (north_star's rtol 1e-3 / atol 1e-5 with margin); bf16 outputs
@@ -33,16 +33,8 @@ def test_gemm_epilogues(capsys):
     _run("probe1", "gemm_epi", capsys, 10)
 
 
-def test_gemm_dynamic_scheduling_is_bit_identical(capsys):
-    _run("probe1", "gemm_clc", capsys, 12)
-
-
 def test_decode_gemv(capsys):
     _run("probe1", "gemv", capsys, 6)
-
-
-def test_gemm_cta_pair_kernel(capsys):
-    _run("probe1", "gemm_2cta", capsys, 24)
 
 
 def test_gemm_fused_gate_up_swiglu(capsys):

@@ -2,7 +2,8 @@
   * against the committed golden fixtures generated from the reference's own modules (tests/golden/make_golden.py);
   * against the installed `transformers` implementations the reference delegates to (CLIPVisionModel, Dinov2Model,
     LlamaDecoderLayer + LlamaRMSNorm + rotary embedding);
-  * directly against the reference modules when /root/reference is present (build container only)."""
+  * against stored outputs (and sampled gradients) of the reference modules in the configurations below
+    (tests/golden/pin_*.npz, same generator)."""
 import os
 import sys
 
@@ -12,10 +13,11 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
-from make_golden import SVA_CASES, SVA_FULL_CASES, SVA_SEP_CASES, seeded_fill, seeded_inputs  # noqa: E402
+from make_golden import (SEP_LIVE_CASES, SVA_CASES, SVA_FULL_CASES, SVA_SEP_CASES, TWO_GROUPS, config1_inputs,  # noqa: E402
+                         flat_sample, grad_sample_index, projector_input, sd_from_layout, seeded_fill, seeded_inputs,
+                         sep_live_dy, two_groups_inputs)
 
 from oracle import cambrian_oracle as O  # noqa: E402
-from oracle import ref_shim  # noqa: E402
 
 GOLD = os.path.join(HERE, "golden")
 
@@ -73,27 +75,26 @@ def test_sva_sep_oracle_matches_reference_golden(name):
     torch.testing.assert_close(got, torch.from_numpy(z["out"]), rtol=1e-4, atol=1e-5)
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="/root/reference not present (GPU box)")
-@pytest.mark.parametrize("rs,q_dim,layers", [([1, 2, 1], 256, 2), ([3], 512, 1), ([1], 1024, 1)])
+@pytest.mark.parametrize("rs,q_dim,layers", SEP_LIVE_CASES)
 def test_sva_sep_oracle_matches_live_reference_fwd_bwd(rs, q_dim, layers):
-    """Output AND gradients of the sep restatement against the live reference module."""
-    vs = ref_shim.ref_module("cambrian.model.vision_sampler")
-    T = len(rs)
-    m = vs.VisionTokenSampler(q_dim, 1024, [1024] * T, rs, 1024, layers, layer_type="sep")
-    m.load_state_dict(seeded_fill(m, 71))
+    """Output AND gradients of the sep restatement against the reference module's (output: a fixed sample plus every row
+    sum; gradients: a fixed sample of every tensor plus its norm; tests/golden/pin_sep_fwd_bwd.npz)."""
+    case = SEP_LIVE_CASES.index((rs, q_dim, layers))
+    z = np.load(os.path.join(GOLD, "pin_sep_fwd_bwd.npz"))
+    zc = {k[len(f"c{case}_"):]: z[k] for k in z.files if k.startswith(f"c{case}_")}
+    sd = {k: v.requires_grad_() for k, v in sd_from_layout(zc, 71).items()}
+    names = [str(k) for k in zc["names"]]
     queries, ctx, feats, masks = seeded_inputs(72, 10, q_dim, rs)
     queries.requires_grad_()
-    ref = m(queries, ctx, *feats, *masks)
-    dy = torch.randn_like(ref)
-    names = [k for k, _ in m.named_parameters()]
-    gref = torch.autograd.grad(ref, [queries] + [p for _, p in m.named_parameters()], dy)
-    sd = {k: v.detach().clone().requires_grad_() for k, v in m.state_dict().items()}
-    q2 = queries.detach().clone().requires_grad_()
-    got = O.sva_sampler(sd, "", q2, ctx, feats, masks, layers, layer_type="sep")
-    ggot = torch.autograd.grad(got, [q2] + [sd[k] for k in names], dy)
-    torch.testing.assert_close(got, ref, rtol=1e-4, atol=1e-5)
-    for a, b, k in zip(ggot, gref, ["queries"] + names):
-        torch.testing.assert_close(a, b, rtol=1e-3, atol=1e-5, msg=lambda s_, k=k: f"{k}: {s_}")
+    got = O.sva_sampler(sd, "", queries, ctx, feats, masks, layers, layer_type="sep")
+    ggot = torch.autograd.grad(got, [queries] + [sd[k] for k in names], sep_live_dy(got.shape))
+    torch.testing.assert_close(flat_sample(got.detach()), torch.from_numpy(zc["out"]), rtol=1e-4, atol=1e-5)
+    torch.testing.assert_close(got.detach().sum(-1), torch.from_numpy(zc["outsum"]), rtol=1e-4, atol=1e-4)
+    idx = grad_sample_index([g.numel() for g in ggot])
+    sample = torch.cat([g.reshape(-1)[torch.from_numpy(ix)] for g, ix in zip(ggot, idx)])
+    torch.testing.assert_close(sample, torch.from_numpy(zc["gsample"]), rtol=1e-3, atol=1e-5)
+    norms = torch.tensor([g.double().norm().item() for g in ggot], dtype=torch.float64)
+    torch.testing.assert_close(norms, torch.from_numpy(zc["gnorm"]), rtol=1e-3, atol=1e-6)
 
 
 @pytest.mark.parametrize("name", sorted(SVA_FULL_CASES))
@@ -179,105 +180,44 @@ def test_oracle_llama_layer_matches_transformers():
     torch.testing.assert_close(got[keymask], ref[keymask], rtol=1e-4, atol=1e-5)
 
 
-# ---------------------------------------------------------------------------------------------- reference present
-needs_ref = pytest.mark.skipif(not ref_shim.available(), reason="/root/reference not present (GPU box)")
-
-
-@needs_ref
+# ------------------------------------------------------------------ stored outputs of the reference modules (pin_*.npz)
 def test_oracle_sva_config1_full_size_against_reference():
-    """BASELINE config 1: SVA projector alone (576 queries, 4 x 24 x 24 x 1024 grids), plus the [1,1,1,4] variant."""
-    vs = ref_shim.ref_module("cambrian.model.vision_sampler")
-    for rs in ([1, 1, 1, 1], [1, 1, 1, 4]):
-        torch.manual_seed(0)
-        m = vs.VisionTokenSampler(1024, 1024, [1024] * 4, rs, 1024, 3).eval()
-        feats = [torch.randn(1, (24 * r) ** 2, 1024) for r in rs]
-        query = (torch.randn(1, 1024) / 32).view(1, 1, 1, -1).expand(1, 576, -1, -1).flatten(0, 1)
-        ctx = feats[0].mean(1).view(1, 1, 1, -1).expand(-1, 576, 1, -1).flatten(0, 1)
-        fw = [O.window_rearrange(f, 24) for f in feats]
-        masks = [torch.rand(576, r * r) > 0.2 for r in rs]
-        for mk in masks:
-            mk[mk.sum(1) == 0] = True
+    """BASELINE config 1: SVA projector alone (576 queries, 4 x 24 x 24 x 1024 grids), plus the [1,1,1,4] variant, with
+    random window masks: a fixed sample of the output and all row sums of the reference module."""
+    z = np.load(os.path.join(GOLD, "pin_config1.npz"))
+    for j, rs in enumerate(([1, 1, 1, 1], [1, 1, 1, 4])):
+        zc = {k[3:]: z[k] for k in z.files if k.startswith(f"r{j}_")}
+        query, ctx, fw, masks = config1_inputs(rs, 82 + j)
         with torch.no_grad():
-            ref = m(query, ctx, *fw, *masks)
-            got = O.sva_sampler(dict(m.state_dict()), "", query, ctx, fw, masks, 3)
-        torch.testing.assert_close(got, ref, rtol=1e-4, atol=2e-5)
+            got = O.sva_sampler(sd_from_layout(zc, 81 + j), "", query, ctx, fw, masks, 3)[:, 0]
+        torch.testing.assert_close(flat_sample(got, 512), torch.from_numpy(zc["sample"]), rtol=1e-4, atol=2e-5)
+        torch.testing.assert_close(got.sum(1), torch.from_numpy(zc["rowsum"]), rtol=1e-4, atol=2e-3)
 
 
-@needs_ref
 def test_oracle_two_query_groups_static_branch_against_reference():
     """cambrian_arch.py:382-420 with num_query_group = 2 (a 4x4 and a 2x2 group: own sampler each, window masks reused
     through the raw reshape of :284, the small group's output bilinearly resized to the final grid :394-401, channel concat,
-    mm_projector, newline column) — the reference's own prepare_inputs_labels_for_multimodal on its static (XLA) branch vs
-    oracle.connector + splice."""
-    import torch.nn as nn
-    vs = ref_shim.ref_module("cambrian.model.vision_sampler")
-    arch = ref_shim.ref_module("cambrian.model.cambrian_arch")
-    H, q, sides, dims = 64, 4, [4, 8], [48, 40]
-
-    class Inner(nn.Module):
-        def __init__(self):
-            super().__init__()
-            for i, c in enumerate(dims):
-                setattr(self, f"mm_projector_aux_{i}", nn.Sequential(nn.Linear(c, 1024), nn.GELU(), nn.Linear(1024, 1024),
-                                                                     nn.LayerNorm(1024)))
-            self.vision_sampler_0 = vs.VisionTokenSampler(1024, 1024, [1024, 1024], [s // 4 for s in sides], 1024, 2)
-            self.vision_sampler_1 = vs.VisionTokenSampler(1024, 1024, [1024, 1024], [s // 2 for s in sides], 1024, 2)
-            self.mm_projector = nn.Sequential(nn.Linear(2048, H), nn.GELU(), nn.Linear(H, H))
-            self.embed_tokens = nn.Embedding(100, H)
-            self.vision_query = nn.Parameter(torch.randn(2, 1024) / 32)
-            self.image_newline = nn.Parameter(torch.randn(H) / 8)
-            self.config = type("C", (), dict(image_token_len=q * q, query_num_list=[q * q, 4], mm_projector_type="sva"))()
-
-        def get_vision_tower_aux_list(self):
-            return [lambda x: x for _ in dims]
-
-    class Top(nn.Module, arch.CambrianMetaForCausalLM):
-        def __init__(self):
-            nn.Module.__init__(self)
-            self.model = Inner()
-            self.config = self.model.config
-            self.device = torch.device("cpu")
-
-        def get_model(self):
-            return self.model
-
-    torch.manual_seed(0)
-    top = Top().eval()
-    B = 2
-    feats = [torch.randn(B, s * s, c) for s, c in zip(sides, dims)]
-    masks = [torch.ones(B * q * q, (s // q) ** 2, dtype=torch.bool) for s in sides]
-    masks[1][::5, 1] = False
-    span = q * (q + 1)
-    ids = torch.randint(3, 100, (B, 5 + span + 6))
-    ids[:, 5] = -200
-    ids[:, 6:5 + span] = 0
-    flag = arch.IS_XLA_AVAILABLE
-    arch.IS_XLA_AVAILABLE = True
-    try:
-        with torch.no_grad():
-            out = top.prepare_inputs_labels_for_multimodal(ids, None, None, None, None, feats, masks, None)
-    finally:
-        arch.IS_XLA_AVAILABLE = flag
-    ref_emb = out[4]
-    sd = {"model." + k: v for k, v in top.model.state_dict().items()}
-    cfg = dict(image_token_len=q * q, query_num_list=[q * q, 4], connector_depth=2)
+    mm_projector, newline column) — the stored result of the reference's own prepare_inputs_labels_for_multimodal on its
+    static (XLA) branch vs oracle.connector + splice."""
+    c = TWO_GROUPS
+    z = np.load(os.path.join(GOLD, "pin_two_groups.npz"))
+    sd = {"model." + k: v for k, v in sd_from_layout(z, c["seed"]).items()}
+    feats, masks, ids = two_groups_inputs()
+    cfg = dict(image_token_len=c["q"] ** 2, query_num_list=[c["q"] ** 2, 4], connector_depth=2)
     with torch.no_grad():
         img, feats_w, ctx_q = O.connector(sd, cfg, feats, masks)
         got = O.splice(sd, ids, img)
-    torch.testing.assert_close(got, ref_emb, rtol=1e-4, atol=2e-5)
-    for a, b in zip(feats_w, out[6]):               # window-rearranged aux features handed to the in-LLM SVA layers
-        torch.testing.assert_close(a, b, rtol=1e-4, atol=2e-5)
+    torch.testing.assert_close(flat_sample(got), torch.from_numpy(z["emb"]), rtol=1e-4, atol=2e-5)
+    torch.testing.assert_close(got.sum(-1), torch.from_numpy(z["embsum"]), rtol=1e-4, atol=1e-4)
+    for i, a in enumerate(feats_w):                 # window-rearranged aux features handed to the in-LLM SVA layers
+        torch.testing.assert_close(flat_sample(a), torch.from_numpy(z[f"feat_w{i}"]), rtol=1e-4, atol=2e-5)
 
 
-@needs_ref
 def test_oracle_projectors_against_reference():
-    pb = ref_shim.ref_module("cambrian.model.multimodal_projector.builder")
-    from helpers import ns
-    torch.manual_seed(0)
-    proj = pb.build_vision_projector(ns(mm_projector_type="mlp2x_gelu", mm_hidden_size=96, hidden_size=64)).eval()
-    x = torch.randn(3, 7, 96)
+    z = np.load(os.path.join(GOLD, "pin_projector.npz"))
+    sd = {"p." + k: v for k, v in sd_from_layout(z, 95).items()}
     with torch.no_grad():
-        torch.testing.assert_close(O.mlp2x_gelu({"p." + k: v for k, v in proj.state_dict().items()}, "p.", x), proj(x),
+        torch.testing.assert_close(flat_sample(O.mlp2x_gelu(sd, "p.", projector_input())), torch.from_numpy(z["out"]),
                                    rtol=1e-5, atol=1e-6)
 
 

@@ -99,32 +99,6 @@ def group_gemm_epi():
     gemm_case(77, 50, 64, False, False, 0, bias=True, residual=True)  # scalar (non-vector) store path
 
 
-def group_gemm_2cta():
-    """CTA-pair kernel (force_bn=512): all operand layouts, tails, epilogues, then throughput vs the single-CTA kernel."""
-    for a_mn in (False, True):
-        for b_mn in (False, True):
-            gemm_case(512, 512, 256, a_mn, b_mn, 512, fp32=True)
-    for (M, N, K) in [(256, 256, 64), (1000, 768, 520), (2304, 1024, 2048), (4096, 4096, 4096), (300, 520, 72)]:
-        for a_mn, b_mn in ((False, False), (False, True), (True, False), (True, True)):
-            if (a_mn and M % 8) or (b_mn and N % 8):
-                continue
-            gemm_case(M, N, K, a_mn, b_mn, 512, fp32=True)
-    gemm_case(512, 768, 512, False, False, 512, batch=3, fp32=True)
-    gemm_case(512, 1024, 512, False, False, 512, bias=True, act="gelu", residual=True)
-    gemm_case(512, 1024, 512, True, True, 512, accumulate=True)
-    for (M, N, K) in [(8192, 8192, 8192), (8192, 28672, 4096), (8192, 4096, 14336), (8192, 6144, 4096)]:
-        for a_mn, b_mn in ((False, False), (False, True), (True, True)):
-            a = torch.randn((K, M) if a_mn else (M, K), device=dev).bfloat16()
-            b = torch.randn((K, N) if b_mn else (N, K), device=dev).bfloat16()
-            out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-            for bn in (256, 512):
-                ms = timeit(lambda: ops.gemm(a, b, a_mn=a_mn, b_mn=b_mn, out=out, force_bn=bn))
-                print(f"perf gemm M={M} N={N} K={K} a_mn={int(a_mn)} b_mn={int(b_mn)} bn={bn}: {ms:.4f} ms "
-                      f"{2 * M * N * K / ms / 1e9:.1f} TFLOP/s", flush=True)
-        ms = timeit(lambda: torch.matmul(a if not a_mn else a.t(), (b.t() if not b_mn else b), out=out))
-        print(f"perf cublas M={M} N={N} K={K}: {ms:.4f} ms {2 * M * N * K / ms / 1e9:.1f} TFLOP/s", flush=True)
-
-
 def group_gemm_swiglu():
     """Fused gate/up projection + SwiGLU (cb_gemm_swiglu_bf16) vs GEMM + the stand-alone SwiGLU kernel and fp32 torch."""
     import torch.nn.functional as F_
@@ -157,64 +131,9 @@ def group_gemm_swiglu():
           f"unfused {t_u:.4f} ms", flush=True)
 
 
-def group_gemm_clc():
-    """Cluster-Launch-Control tile scheduling vs the static persistent walk: bit-identical outputs for every kernel variant
-    (single CTA BN 64/128/256, CTA pair, every operand major, batched, accumulate, fused SwiGLU), alone and while another
-    stream keeps the SMs busy (the situation it exists for); then the timing of both."""
-    cases = [  # M, N, K, a_mn, b_mn, force_bn, batch
-        (4096, 4096, 512, False, False, 64, 0), (4096, 4096, 1024, False, False, 128, 0), (8192, 4096, 512, False, False, 256, 0),
-        (8192, 8192, 1024, False, False, 512, 0), (4096, 4096, 2048, False, True, 512, 0), (4096, 4096, 2048, True, True, 512, 0),
-        (4096, 4096, 2048, True, False, 128, 0), (2048, 1024, 256, False, False, 64, 6), (8200, 4104, 264, False, False, 0, 0),
-        (4096, 1024, 8192, True, True, 0, 0), (8192, 14336, 4096, False, True, 0, 0)]
-    hog_a = torch.randn(64 << 20, device=dev)
-    side = torch.cuda.Stream()
-    for (M, N, K, a_mn, b_mn, bn, batch) in cases:
-        bs = (batch,) if batch else ()
-        a = torch.randn(*bs, *((K, M) if a_mn else (M, K)), device=dev).bfloat16()
-        b = torch.randn(*bs, *((K, N) if b_mn else (N, K)), device=dev).bfloat16()
-        acc0 = torch.randn(*bs, M, N, device=dev).bfloat16()
-        outs = []
-        for mode in (0, 1, 2):                 # static, CLC, CLC under contention
-            ops.gemm_set_dynamic_scheduling(mode > 0)
-            if mode == 2:
-                side.wait_stream(torch.cuda.current_stream())
-                with torch.cuda.stream(side):
-                    for _ in range(6):
-                        hog_a.mul_(1.0001)     # 256 MB elementwise passes: every SM's thread slots taken in bursts
-            o1 = ops.gemm(a, b, a_mn=a_mn, b_mn=b_mn, force_bn=bn)
-            o2 = ops.gemm(a, b, a_mn=a_mn, b_mn=b_mn, force_bn=bn, out=acc0.clone(), accumulate=True)
-            o3 = ops.gemm(a, b, a_mn=a_mn, b_mn=b_mn, force_bn=bn, out_dtype=torch.float32)
-            torch.cuda.synchronize()
-            outs.append((o1, o2, o3))
-        same = all(torch.equal(x, y) for m in (1, 2) for x, y in zip(outs[0], outs[m]))
-        A = a.float().transpose(-1, -2) if a_mn else a.float()
-        B = b.float() if b_mn else b.float().transpose(-1, -2)
-        e = rel_err(outs[1][2], A @ B)
-        print(f"clc M={M} N={N} K={K} a_mn={int(a_mn)} b_mn={int(b_mn)} bn={bn} batch={batch}: identical={same} fp32 err {e:.2e}"
-              f" {'OK' if same and e < 2e-5 else 'FAIL'}")
-    x = torch.randn(8192, 4096, device=dev).bfloat16()
-    w = torch.randn(2 * 14336, 4096, device=dev).bfloat16() * 0.02
-    res = []
-    for mode in (0, 1):
-        ops.gemm_set_dynamic_scheduling(bool(mode))
-        res.append(ops.gemm_swiglu(x, w))
-        torch.cuda.synchronize()
-    same = torch.equal(res[0][0], res[1][0]) and torch.equal(res[0][1], res[1][1])
-    print(f"clc fused gate/up + SwiGLU M=8192 F=14336 K=4096: identical={same} {'OK' if same else 'FAIL'}")
-    for (M, N, K) in ((8192, 28672, 4096), (8192, 4096, 14336), (8192, 6144, 4096), (4096, 1024, 1024), (2304, 1024, 1024)):
-        a = torch.randn(M, K, device=dev).bfloat16()
-        b = torch.randn(N, K, device=dev).bfloat16()
-        t = []
-        for mode in (0, 1):
-            ops.gemm_set_dynamic_scheduling(bool(mode))
-            t.append(timeit(lambda: ops.gemm(a, b)))
-        print(f"clc timing M={M} N={N} K={K}: static {2 * M * N * K / t[0] / 1e9:7.0f} TF/s  dynamic {2 * M * N * K / t[1] / 1e9:7.0f} TF/s")
-    ops.gemm_set_dynamic_scheduling(True)
-
-
 def group_gemv():
     """Decode-shaped (M <= 8) projections: the weight-streaming GEMV vs an fp32 reference (bias / residual / fp32 output /
-    ragged N and K tails), and the achieved weight bandwidth of GEMV and of the 128-row tcgen05 tile on the same shapes."""
+    ragged N and K tails), and the achieved weight bandwidth of GEMV and of the 128-row wgmma tile on the same shapes."""
     for (M, N, K, bias, res, f32) in [(1, 4096, 4096, False, True, False), (3, 520, 1032, True, False, False),
                                       (8, 6144, 4096, False, False, False), (5, 1000, 2056, True, True, True),
                                       (8, 128256, 4096, False, False, True), (2, 4096, 14336, False, True, False)]:
@@ -239,7 +158,7 @@ def group_gemv():
             ops._GEMV = False
             t_t = timeit(lambda: ops.gemm(x, w), iters=30)
             ops._GEMV = True
-            print(f"gemv perf M={M} N={N} K={K}: gemv {t_v * 1e3:7.1f} us {N * K * 2 / t_v / 1e6:6.0f} GB/s | tcgen05 tile "
+            print(f"gemv perf M={M} N={N} K={K}: gemv {t_v * 1e3:7.1f} us {N * K * 2 / t_v / 1e6:6.0f} GB/s | wgmma tile "
                   f"{t_t * 1e3:7.1f} us {N * K * 2 / t_t / 1e6:6.0f} GB/s", flush=True)
 
 

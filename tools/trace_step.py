@@ -2,7 +2,7 @@
 
     python -m torch.distributed.run --nproc-per-node N ... tools/trace_step.py --gpus N [--config 8b-ddp]
 
-Rank 0 writes gpurun_out/trace_n{N}.json: per stream {kernels, busy ms, first/last}, the NCCL kernels (count, total ms, how
+Rank 0 writes trace_out/trace_n{N}.json: per stream {kernels, busy ms, first/last}, the NCCL kernels (count, total ms, how
 much of that time a compute kernel was running on another stream = overlapped), main-stream idle gaps, and the step wall
 time.  This is the evidence for 'the collectives hide under backward' (or not)."""
 import argparse
@@ -89,8 +89,8 @@ def main():
             dist.barrier()
             dist.destroy_process_group()
         return
-    os.makedirs("gpurun_out", exist_ok=True)
-    path = f"gpurun_out/trace_n{world}_raw.json"
+    os.makedirs("trace_out", exist_ok=True)
+    path = f"trace_out/trace_n{world}_raw.json"
     prof.export_chrome_trace(path)
     ev = [e for e in json.load(open(path))["traceEvents"] if e.get("cat") == "kernel"]
     with gzip.open(path + ".gz", "wt") as f:
@@ -121,7 +121,7 @@ def main():
                                       first_ms=(min(e["ts"] for e in v) - t0) / 1e3,
                                       last_ms=(max(e["ts"] + e["dur"] for e in v) - t0) / 1e3,
                                       top=sorted({e["name"][:50] for e in v})[:3]) for s, v in streams.items()})
-    json.dump(summ, open(f"gpurun_out/trace_n{world}.json", "w"), indent=1)
+    json.dump(summ, open(f"trace_out/trace_n{world}.json", "w"), indent=1)
     print(json.dumps({k: v for k, v in summ.items() if k != "streams"}))
     if world > 1:
         dist.barrier()
