@@ -42,7 +42,7 @@ struct GemmEpilogue {
   void* aux;       // fused SwiGLU: second output, silu(gate) * up, [M, N / 2] bf16
   long long ld_aux;
 };
-constexpr int ACT_SWIGLU_PAIR = 5;  // the tile's two B halves are 64 gate rows and the matching 64 up rows
+constexpr int ACT_SWIGLU_PAIR = 5;  // the tile's two B halves are BN / 2 gate rows and the matching BN / 2 up rows
 
 template <int BN>
 struct GemmCfg {
@@ -76,52 +76,101 @@ __device__ __forceinline__ void tile_to_mn(int r, int m_blocks, int n_blocks, in
   nb = w / gs;
 }
 
-// one output element pair (columns col, col + 1 of one row): alpha, bias, activation, LayerScale, residual, accumulate
+// One accumulator row of the tile, this thread's BN / 4 columns (pairs col0 + 8 j, + 1): alpha, bias, activation,
+// LayerScale, residual, accumulate, store.  Each fusion is one pass over the row under one test of its flag, so that its
+// loads are issued together and no load waits behind a store; the element-wise order of operations is the same in every
+// pass.  Needs ep.pair_ok: N is even, so col + 1 < N whenever col < N.
+template <int BN, int ACT>
+__device__ __forceinline__ void epilogue_row(const GemmEpilogue& ep, long long c_off, long long r_off, int col0, int N,
+                                             const float* acc, int h) {
+  constexpr int J = BN / 8;
+  float2 v[J];
+#pragma unroll
+  for (int j = 0; j < J; ++j) v[j] = make_float2(acc[4 * j + 2 * h] * ep.alpha, acc[4 * j + 2 * h + 1] * ep.alpha);
+  if (ep.bias) {
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      const int col = col0 + 8 * j;
+      if (col < N) {
+        const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ep.bias + col));
+        v[j].x += t.x;
+        v[j].y += t.y;
+      }
+    }
+  }
+  if constexpr (ACT != 0) {
+#pragma unroll
+    for (int j = 0; j < J; ++j) v[j] = make_float2(apply_act<ACT>(v[j].x), apply_act<ACT>(v[j].y));
+  }
+  if (ep.colscale) {
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      const int col = col0 + 8 * j;
+      if (col < N) {
+        const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ep.colscale + col));
+        v[j].x *= t.x;
+        v[j].y *= t.y;
+      }
+    }
+  }
+  if (ep.residual) {
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      const int col = col0 + 8 * j;
+      if (col < N) {
+        const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ep.residual + r_off + col));
+        v[j].x += t.x;
+        v[j].y += t.y;
+      }
+    }
+  }
+  if (ep.out_fp32) {
+    float* cr = reinterpret_cast<float*>(ep.C) + c_off;
+    if (ep.accumulate) {
+#pragma unroll
+      for (int j = 0; j < J; ++j) {
+        const int col = col0 + 8 * j;
+        if (col < N) {
+          const float2 o = *reinterpret_cast<const float2*>(cr + col);
+          v[j].x += o.x;
+          v[j].y += o.y;
+        }
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      const int col = col0 + 8 * j;
+      if (col < N) *reinterpret_cast<float2*>(cr + col) = v[j];
+    }
+  } else {
+    bf16* cr = reinterpret_cast<bf16*>(ep.C) + c_off;
+    if (ep.accumulate) {
+#pragma unroll
+      for (int j = 0; j < J; ++j) {
+        const int col = col0 + 8 * j;
+        if (col < N) {
+          const float2 o = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(cr + col));
+          v[j].x += o.x;
+          v[j].y += o.y;
+        }
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      const int col = col0 + 8 * j;
+      if (col < N) *reinterpret_cast<__nv_bfloat162*>(cr + col) = __floats2bfloat162_rn(v[j].x, v[j].y);
+    }
+  }
+}
+
+// odd N or a misaligned operand: the same operations element by element (columns col, col + 1 of one row)
 template <int ACT>
-__device__ __forceinline__ void epilogue_pair(const GemmEpilogue& ep, long long c_off, long long r_off, int col, int N,
-                                              float v0, float v1) {
+__device__ __forceinline__ void epilogue_elems(const GemmEpilogue& ep, long long c_off, long long r_off, int col, int N,
+                                               float v0, float v1) {
   v0 *= ep.alpha;
   v1 *= ep.alpha;
-  if (ep.pair_ok) {
-    if (col >= N) return;  // N is even here, so col + 1 < N as well
-    if (ep.bias) {
-      const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ep.bias + col));
-      v0 += t.x;
-      v1 += t.y;
-    }
-    v0 = apply_act<ACT>(v0);
-    v1 = apply_act<ACT>(v1);
-    if (ep.colscale) {
-      const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ep.colscale + col));
-      v0 *= t.x;
-      v1 *= t.y;
-    }
-    if (ep.residual) {
-      const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ep.residual + r_off + col));
-      v0 += t.x;
-      v1 += t.y;
-    }
-    if (ep.out_fp32) {
-      float2* cp = reinterpret_cast<float2*>(reinterpret_cast<float*>(ep.C) + c_off + col);
-      if (ep.accumulate) {
-        const float2 o = *cp;
-        v0 += o.x;
-        v1 += o.y;
-      }
-      *cp = make_float2(v0, v1);
-    } else {
-      __nv_bfloat162* cp = reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<bf16*>(ep.C) + c_off + col);
-      if (ep.accumulate) {
-        const float2 o = __bfloat1622float2(*cp);
-        v0 += o.x;
-        v1 += o.y;
-      }
-      *cp = __floats2bfloat162_rn(v0, v1);
-    }
-    return;
-  }
 #pragma unroll
-  for (int e = 0; e < 2; ++e) {  // odd N or a misaligned operand: element by element
+  for (int e = 0; e < 2; ++e) {
     const int c = col + e;
     if (c >= N) break;
     float v = e ? v1 : v0;
@@ -155,9 +204,9 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  // SwiGLU: N = 2F columns, one tile = 64 features (64 gate + 64 up columns)
+  // SwiGLU: N = 2F columns, one tile = BN / 2 features (BN / 2 gate + BN / 2 up columns)
   const int m_blocks = (M + BM - 1) / BM;
-  const int n_blocks = SWIGLU ? (N / 2) / 64 : (N + BN - 1) / BN;
+  const int n_blocks = SWIGLU ? (N / 2) / (BN / 2) : (N + BN - 1) / BN;
   const int tiles_per_batch = m_blocks * n_blocks;
   const int b = blockIdx.x / tiles_per_batch;
   int mb, nb;
@@ -193,9 +242,9 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 #pragma unroll
           for (int i = 0; i < BM / 64; ++i) tma_load_3d(sa + i * (64 * BK * 2), &tmA, full_bar(stage), m0 + 64 * i, k0, b);
         }
-        if (SWIGLU) {  // gate rows [64 nb, +64) and up rows [F + 64 nb, +64)
-          tma_load_3d(sb, &tmB, full_bar(stage), k0, nb * 64, 0);
-          tma_load_3d(sb + 64 * BK * 2, &tmB, full_bar(stage), k0, N / 2 + nb * 64, 0);
+        if (SWIGLU) {  // gate rows [nb BN/2, +BN/2) and up rows [F + nb BN/2, +BN/2)
+          tma_load_3d(sb, &tmB, full_bar(stage), k0, nb * (BN / 2), 0);
+          tma_load_3d(sb + (BN / 2) * BK * 2, &tmB, full_bar(stage), k0, N / 2 + nb * (BN / 2), 0);
         } else if (!B_MN) {
           tma_load_3d(sb, &tmB, full_bar(stage), k0, nb * BN, b);
         } else {
@@ -252,8 +301,9 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   const int r_lo = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const int cq = 2 * (lane & 3);
   if constexpr (SWIGLU) {
-    // accumulator columns [0, 64) = gate, [64, 128) = up of the same 64 features: write both pre-activations (saved for
-    // backward) and silu(gate) * up without a second pass over the [M, 2F] tensor
+    // accumulator columns [0, BN/2) = gate, [BN/2, BN) = up of the same BN/2 features: write both pre-activations (saved
+    // for backward) and silu(gate) * up without a second pass over the [M, 2F] tensor
+    constexpr int JH = BN / 16;  // 8-column groups per half
     const int F = N >> 1;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -262,11 +312,11 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       bf16* gu = reinterpret_cast<bf16*>(ep.C) + static_cast<long long>(row) * ep.ldc;
       bf16* ao = reinterpret_cast<bf16*>(ep.aux) + static_cast<long long>(row) * ep.ld_aux;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int f = nb * 64 + 8 * j + cq;
+      for (int j = 0; j < JH; ++j) {
+        const int f = nb * (BN / 2) + 8 * j + cq;
         // round to bf16 first: the separate kernels (and the reference) apply silu to the STORED bf16 pre-activations
         const __nv_bfloat162 g2 = __floats2bfloat162_rn(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-        const __nv_bfloat162 u2 = __floats2bfloat162_rn(acc[4 * (j + 8) + 2 * h], acc[4 * (j + 8) + 2 * h + 1]);
+        const __nv_bfloat162 u2 = __floats2bfloat162_rn(acc[4 * (j + JH) + 2 * h], acc[4 * (j + JH) + 2 * h + 1]);
         const float2 g = __bfloat1622float2(g2), u = __bfloat1622float2(u2);
         *reinterpret_cast<__nv_bfloat162*>(gu + f) = g2;
         *reinterpret_cast<__nv_bfloat162*>(gu + F + f) = u2;
@@ -281,11 +331,14 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       if (row >= M) continue;
       const long long c_off = static_cast<long long>(b) * ep.bsc + static_cast<long long>(row) * ep.ldc;
       const long long r_off = static_cast<long long>(b) * ep.bsr + static_cast<long long>(row) * ep.ldr;
+      if (ep.pair_ok) {
+        epilogue_row<BN, ACT>(ep, c_off, r_off, n0 + cq, N, acc, h);
+        continue;
+      }
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
-        const int col = n0 + 8 * j + cq;
         if (n0 + 8 * j >= N) break;
-        epilogue_pair<ACT>(ep, c_off, r_off, col, N, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        epilogue_elems<ACT>(ep, c_off, r_off, n0 + 8 * j + cq, N, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
       }
     }
   }
@@ -348,7 +401,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, in
     if (e != cudaSuccess) return set_error(CB_ERR_CUDA, "gemm smem attr: %s", cudaGetErrorString(e));
     attr_set = true;
   }
-  const int n_blocks = (ACT == ACT_SWIGLU_PAIR) ? (N / 2) / 64 : (N + BN - 1) / BN;
+  const int n_blocks = (ACT == ACT_SWIGLU_PAIR) ? (N / 2) / (BN / 2) : (N + BN - 1) / BN;
   const long long tiles = (long long)((M + BM - 1) / BM) * n_blocks * batch;
   CB_CHECK_ARG(tiles < (1LL << 31), "gemm: %lld tiles exceed the grid", tiles);
   kern<<<(unsigned)tiles, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, M, N, K, ep);
@@ -431,21 +484,24 @@ int gemm_swiglu_bf16(const void* A, const void* W, void* gu_out, void* act_out, 
                      long long ldw, long long ld_gu, long long ld_act, cudaStream_t stream) {
   CB_CHECK_ARG(M > 0 && F > 0 && K > 0, "gemm_swiglu: empty problem M=%d F=%d K=%d", M, F, K);
   CB_CHECK_ARG(A && W && gu_out && act_out, "gemm_swiglu: null operand");
-  CB_CHECK_ARG(F % 128 == 0, "gemm_swiglu: F=%d must be a multiple of 128 (whole 64-feature tiles, 16-byte aligned halves)", F);
+  CB_CHECK_ARG(F % 128 == 0, "gemm_swiglu: F=%d must be a multiple of 128 (whole 128-feature tiles, 16-byte aligned halves)", F);
   CB_CHECK_ARG(ld_gu % 8 == 0 && ld_act % 8 == 0 && ((reinterpret_cast<uintptr_t>(gu_out) & 15u) == 0) &&
                    ((reinterpret_cast<uintptr_t>(act_out) & 15u) == 0),
                "gemm_swiglu: outputs must be 16-byte aligned with ld %% 8 == 0");
   const int N = 2 * F;
+  // 128 gate + 128 up features per tile: the same 128 x 256 tile and operand traffic per FLOP as the generic BN = 256
+  // kernel (a 64 + 64 tile reads 32 KB of operands per 64-deep k-block for half the FLOPs of a 48 KB 128 x 256 k-block)
+  constexpr int BN = 256;
   CUtensorMap tmA, tmB;
   int rc;
   if ((rc = make_tmap_bf16_3d(&tmA, A, K, M, 1, lda, 0, BM))) return rc;
-  if ((rc = make_tmap_bf16_3d(&tmB, W, K, N, 1, ldw, 0, 64))) return rc;
+  if ((rc = make_tmap_bf16_3d(&tmB, W, K, N, 1, ldw, 0, BN / 2))) return rc;
   GemmEpilogue ep;
   ep.C = gu_out; ep.ldc = ld_gu; ep.bsc = 0;
   ep.bias = nullptr; ep.colscale = nullptr; ep.residual = nullptr; ep.ldr = 0; ep.bsr = 0;
   ep.alpha = 1.0f; ep.out_fp32 = 0; ep.accumulate = 0; ep.pair_ok = 1;
   ep.aux = act_out; ep.ld_aux = ld_act;
-  return launch_gemm<128, false, false, ACT_SWIGLU_PAIR>(tmA, tmB, M, N, K, 1, ep, stream);
+  return launch_gemm<BN, false, false, ACT_SWIGLU_PAIR>(tmA, tmB, M, N, K, 1, ep, stream);
 }
 
 }  // namespace cb

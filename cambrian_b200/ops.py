@@ -699,8 +699,9 @@ _FUSED_SWIGLU = os.environ.get("CB_FUSED_SWIGLU", "1") != "0"
 
 
 def mlp_gate_up(h2d, w_gu):
-    """gate/up projection + SwiGLU: the fused kernel (128-row x 64-feature tiles) when the problem fills the SMs for >= 3
-    waves and F % 128 == 0, otherwise GEMM (whose tile width adapts to small problems) followed by the SwiGLU kernel."""
+    """gate/up projection + SwiGLU: the fused kernel (128-row x 128-feature tiles) when the [M, 2F] output holds at least
+    3 x SMs blocks of 128 x 128 and F % 128 == 0, otherwise GEMM (whose tile width adapts to small problems) followed by
+    the SwiGLU kernel."""
     M = h2d.shape[0]
     F2 = w_gu.shape[0]
     I = F2 // 2
