@@ -615,7 +615,7 @@ class DecoderLayerFn(torch.autograd.Function):
     """
 
     @staticmethod
-    def _forward(meta, x, ln1, qkv_w, o_w, ln2, gu_w, down_w, keep):
+    def _forward(meta, x, ln1, qkv_w, o_w, ln2, gu_w, down_w, keep, need_out=True):
         B, S, H = x.shape
         nh, nkv, hd = meta["nh"], meta["nkv"], meta["hd"]
         rows = B * S
@@ -631,10 +631,11 @@ class DecoderLayerFn(torch.autograd.Function):
         x1 = ops.gemm(attn2, o_w, residual=x2)
         h2, rstd2 = ops.rmsnorm_fwd(x1, ln2, meta["eps"], meta["hf_cast"], save_stats=True)
         gu, act = ops.mlp_gate_up(h2, gu_w)
+        saved = (rstd1, qkv, attn, lse, x1, rstd2, gu, act) if keep else None
+        if not need_out:  # the backward's recompute needs only the saved activations, not the layer's output
+            return None, saved
         out = ops.gemm(act, down_w, residual=x1)
-        if keep:
-            return out.view(B, S, H), (rstd1, qkv, attn, lse, x1, rstd2, gu, act)
-        return out.view(B, S, H), None
+        return out.view(B, S, H), saved
 
     @staticmethod
     @_ranged("decoder_layer.fwd")
@@ -659,7 +660,7 @@ class DecoderLayerFn(torch.autograd.Function):
         sv = ctx.saved_tensors
         x, ln1, qkv_w, o_w, ln2, gu_w, down_w = sv[:7]
         if meta["recompute"]:
-            _, saved = DecoderLayerFn._forward(meta, x, ln1, qkv_w, o_w, ln2, gu_w, down_w, True)
+            _, saved = DecoderLayerFn._forward(meta, x, ln1, qkv_w, o_w, ln2, gu_w, down_w, True, need_out=False)
         else:
             saved = sv[7:]
         rstd1, qkv, attn, lse, x1, rstd2, gu, act = saved

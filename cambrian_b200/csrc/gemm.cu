@@ -11,12 +11,17 @@
 // wgmma reads either major straight from shared memory (the transpose bits of the instruction), so no layout
 // needs a transposed copy.
 //
-// Structure (one CTA per 128 x BN output tile, 288 threads):
-//     warp 8      TMA producer   : cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx
+// Structure (persistent: min(tiles, SMs) CTAs of 288 threads, each walking the 128 x BN output tiles
+// r = blockIdx.x, + gridDim.x, ...):
+//     warp 8      TMA producer   : cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx.  The ring's stage and
+//                 phase carry across tiles, so the next tile's first k-blocks load while this tile's epilogue runs.
 //     warps 0..7  two consumer warpgroups, 64 rows each: wgmma.mma_async 64 x BN x 16 with fp32 accumulators in
-//                 registers, one k-block group kept in flight, then bias / act / scale / residual -> HBM
+//                 registers, one k-block group kept in flight, then bias / act / scale / residual in registers and
+//                 the bf16 result through a swizzled smem sub-tile and a TMA store (cp.async.bulk.tensor), which
+//                 completes while the warpgroup already runs the next tile's MMAs.
 // BN = 64 / 128 / 256 is chosen per problem so that small GEMMs still put a CTA on most of the 132 SMs.
 #include "common.cuh"
+#include <algorithm>
 #include <cstring>
 #include <cudaTypedefs.h>
 #include <mutex>
@@ -39,18 +44,23 @@ struct GemmEpilogue {
   int out_fp32;    // C dtype: 0 bf16, 1 fp32
   int accumulate;  // C += result
   int pair_ok;     // two adjacent columns can be loaded / stored as one 4-byte (bf16) / 8-byte (fp32) access
-  void* aux;       // fused SwiGLU: second output, silu(gate) * up, [M, N / 2] bf16
-  long long ld_aux;
+  int tma_store;   // bf16 C addressable by TMA (tmC): stores go through smem; otherwise straight from registers
 };
 constexpr int ACT_SWIGLU_PAIR = 5;  // the tile's two B halves are BN / 2 gate rows and the matching BN / 2 up rows
+
+// epilogue staging: two 64 x 64 bf16 sub-tiles (SWIZZLE_128B, one TMA store box each) per consumer warpgroup, so one
+// can be written while the other's store still reads it
+constexpr int STG_BYTES = 64 * 64 * 2;
+constexpr int STAGING_BYTES = 2 * 2 * STG_BYTES;
 
 template <int BN>
 struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);  // 192 KB of operands at every BN
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
 };
 
 // activation selected at COMPILE time: a per-element runtime switch (plus slow-path erff / tanhf) made the epilogue of
@@ -76,31 +86,37 @@ __device__ __forceinline__ void tile_to_mn(int r, int m_blocks, int n_blocks, in
   nb = w / gs;
 }
 
-// One accumulator row of the tile, this thread's BN / 4 columns (pairs col0 + 8 j, + 1): alpha, bias, activation,
-// LayerScale, residual, accumulate, store.  Each fusion is one pass over the row under one test of its flag, so that its
-// loads are issued together and no load waits behind a store; the element-wise order of operations is the same in every
-// pass.  Needs ep.pair_ok: N is even, so col + 1 < N whenever col < N.
+// One accumulator row of the tile, this thread's BN / 4 columns (pairs col0 + 8 j, + 1), in place: alpha, bias,
+// activation, LayerScale, residual, accumulate (C's old value).  Each fusion is one pass over the row under one test of
+// its flag, so that its loads are issued together and no load waits behind a store; the element-wise order of operations
+// is the same in every pass, and the caller rounds / stores last.  Needs ep.pair_ok: N is even, so col + 1 < N whenever
+// col < N.
 template <int BN, int ACT>
-__device__ __forceinline__ void epilogue_row(const GemmEpilogue& ep, long long c_off, long long r_off, int col0, int N,
-                                             const float* acc, int h) {
+__device__ __forceinline__ void fuse_row(const GemmEpilogue& ep, long long c_off, long long r_off, int col0, int N,
+                                         float* acc, int h) {
   constexpr int J = BN / 8;
-  float2 v[J];
 #pragma unroll
-  for (int j = 0; j < J; ++j) v[j] = make_float2(acc[4 * j + 2 * h] * ep.alpha, acc[4 * j + 2 * h + 1] * ep.alpha);
+  for (int j = 0; j < J; ++j) {
+    acc[4 * j + 2 * h] *= ep.alpha;
+    acc[4 * j + 2 * h + 1] *= ep.alpha;
+  }
   if (ep.bias) {
 #pragma unroll
     for (int j = 0; j < J; ++j) {
       const int col = col0 + 8 * j;
       if (col < N) {
         const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ep.bias + col));
-        v[j].x += t.x;
-        v[j].y += t.y;
+        acc[4 * j + 2 * h] += t.x;
+        acc[4 * j + 2 * h + 1] += t.y;
       }
     }
   }
   if constexpr (ACT != 0) {
 #pragma unroll
-    for (int j = 0; j < J; ++j) v[j] = make_float2(apply_act<ACT>(v[j].x), apply_act<ACT>(v[j].y));
+    for (int j = 0; j < J; ++j) {
+      acc[4 * j + 2 * h] = apply_act<ACT>(acc[4 * j + 2 * h]);
+      acc[4 * j + 2 * h + 1] = apply_act<ACT>(acc[4 * j + 2 * h + 1]);
+    }
   }
   if (ep.colscale) {
 #pragma unroll
@@ -108,8 +124,8 @@ __device__ __forceinline__ void epilogue_row(const GemmEpilogue& ep, long long c
       const int col = col0 + 8 * j;
       if (col < N) {
         const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ep.colscale + col));
-        v[j].x *= t.x;
-        v[j].y *= t.y;
+        acc[4 * j + 2 * h] *= t.x;
+        acc[4 * j + 2 * h + 1] *= t.y;
       }
     }
   }
@@ -119,47 +135,47 @@ __device__ __forceinline__ void epilogue_row(const GemmEpilogue& ep, long long c
       const int col = col0 + 8 * j;
       if (col < N) {
         const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ep.residual + r_off + col));
-        v[j].x += t.x;
-        v[j].y += t.y;
+        acc[4 * j + 2 * h] += t.x;
+        acc[4 * j + 2 * h + 1] += t.y;
       }
     }
   }
-  if (ep.out_fp32) {
-    float* cr = reinterpret_cast<float*>(ep.C) + c_off;
-    if (ep.accumulate) {
-#pragma unroll
-      for (int j = 0; j < J; ++j) {
-        const int col = col0 + 8 * j;
-        if (col < N) {
-          const float2 o = *reinterpret_cast<const float2*>(cr + col);
-          v[j].x += o.x;
-          v[j].y += o.y;
-        }
-      }
-    }
+  if (ep.accumulate && ep.out_fp32) {
+    const float* cr = reinterpret_cast<const float*>(ep.C) + c_off;
 #pragma unroll
     for (int j = 0; j < J; ++j) {
       const int col = col0 + 8 * j;
-      if (col < N) *reinterpret_cast<float2*>(cr + col) = v[j];
-    }
-  } else {
-    bf16* cr = reinterpret_cast<bf16*>(ep.C) + c_off;
-    if (ep.accumulate) {
-#pragma unroll
-      for (int j = 0; j < J; ++j) {
-        const int col = col0 + 8 * j;
-        if (col < N) {
-          const float2 o = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(cr + col));
-          v[j].x += o.x;
-          v[j].y += o.y;
-        }
+      if (col < N) {
+        const float2 o = *reinterpret_cast<const float2*>(cr + col);
+        acc[4 * j + 2 * h] += o.x;
+        acc[4 * j + 2 * h + 1] += o.y;
       }
     }
+  } else if (ep.accumulate) {
+    const bf16* cr = reinterpret_cast<const bf16*>(ep.C) + c_off;
 #pragma unroll
     for (int j = 0; j < J; ++j) {
       const int col = col0 + 8 * j;
-      if (col < N) *reinterpret_cast<__nv_bfloat162*>(cr + col) = __floats2bfloat162_rn(v[j].x, v[j].y);
+      if (col < N) {
+        const float2 o = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(cr + col));
+        acc[4 * j + 2 * h] += o.x;
+        acc[4 * j + 2 * h + 1] += o.y;
+      }
     }
+  }
+}
+
+// the register-path store of a row fused by fuse_row (fp32 C, or bf16 C that TMA cannot address)
+template <int BN>
+__device__ __forceinline__ void store_row(const GemmEpilogue& ep, long long c_off, int col0, int N, const float* acc,
+                                          int h) {
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = col0 + 8 * j;
+    if (col >= N) continue;
+    const float x = acc[4 * j + 2 * h], y = acc[4 * j + 2 * h + 1];
+    if (ep.out_fp32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(ep.C) + c_off + col) = make_float2(x, y);
+    else *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<bf16*>(ep.C) + c_off + col) = __floats2bfloat162_rn(x, y);
   }
 }
 
@@ -190,15 +206,17 @@ __device__ __forceinline__ void epilogue_elems(const GemmEpilogue& ep, long long
 
 template <int BN, bool A_MN, bool B_MN, int ACT>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K,
-                GemmEpilogue ep) {
+gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAux, int M, int N, int K,
+                int tiles, GemmEpilogue ep) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   constexpr bool SWIGLU = ACT == ACT_SWIGLU_PAIR;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte aligned bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
+  const uint32_t stg_base = smem_base + STAGES * Cfg::STAGE_BYTES;
+  const uint32_t bar_base = stg_base + STAGING_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
 
@@ -208,10 +226,6 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   const int m_blocks = (M + BM - 1) / BM;
   const int n_blocks = SWIGLU ? (N / 2) / (BN / 2) : (N + BN - 1) / BN;
   const int tiles_per_batch = m_blocks * n_blocks;
-  const int b = blockIdx.x / tiles_per_batch;
-  int mb, nb;
-  tile_to_mn(blockIdx.x - b * tiles_per_batch, m_blocks, n_blocks, mb, nb);
-  const int m0 = mb * BM;
   const int num_kb = (K + BK - 1) / BK;
 
   if (warp == 8 && lane == 0) {
@@ -230,31 +244,38 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(empty_bar(stage), phase ^ 1u);
-        const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-        const uint32_t sb = sa + Cfg::A_BYTES;
-        mbar_arrive_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
-        const int k0 = kb * BK;
-        if (!A_MN) {
-          tma_load_3d(sa, &tmA, full_bar(stage), k0, m0, b);
-        } else {
+      for (int r = blockIdx.x; r < tiles; r += gridDim.x) {
+        const int b = r / tiles_per_batch;
+        int mb, nb;
+        tile_to_mn(r - b * tiles_per_batch, m_blocks, n_blocks, mb, nb);
+        const int m0 = mb * BM;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(empty_bar(stage), phase ^ 1u);
+          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
+          const uint32_t sb = sa + Cfg::A_BYTES;
+          mbar_arrive_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
+          const int k0 = kb * BK;
+          if (!A_MN) {
+            tma_load_3d(sa, &tmA, full_bar(stage), k0, m0, b);
+          } else {
 #pragma unroll
-          for (int i = 0; i < BM / 64; ++i) tma_load_3d(sa + i * (64 * BK * 2), &tmA, full_bar(stage), m0 + 64 * i, k0, b);
-        }
-        if (SWIGLU) {  // gate rows [nb BN/2, +BN/2) and up rows [F + nb BN/2, +BN/2)
-          tma_load_3d(sb, &tmB, full_bar(stage), k0, nb * (BN / 2), 0);
-          tma_load_3d(sb + (BN / 2) * BK * 2, &tmB, full_bar(stage), k0, N / 2 + nb * (BN / 2), 0);
-        } else if (!B_MN) {
-          tma_load_3d(sb, &tmB, full_bar(stage), k0, nb * BN, b);
-        } else {
+            for (int i = 0; i < BM / 64; ++i)
+              tma_load_3d(sa + i * (64 * BK * 2), &tmA, full_bar(stage), m0 + 64 * i, k0, b);
+          }
+          if (SWIGLU) {  // gate rows [nb BN/2, +BN/2) and up rows [F + nb BN/2, +BN/2)
+            tma_load_3d(sb, &tmB, full_bar(stage), k0, nb * (BN / 2), 0);
+            tma_load_3d(sb + (BN / 2) * BK * 2, &tmB, full_bar(stage), k0, N / 2 + nb * (BN / 2), 0);
+          } else if (!B_MN) {
+            tma_load_3d(sb, &tmB, full_bar(stage), k0, nb * BN, b);
+          } else {
 #pragma unroll
-          for (int i = 0; i < BN / 64; ++i)
-            tma_load_3d(sb + i * (64 * BK * 2), &tmB, full_bar(stage), nb * BN + 64 * i, k0, b);
-        }
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1u;
+            for (int i = 0; i < BN / 64; ++i)
+              tma_load_3d(sb + i * (64 * BK * 2), &tmB, full_bar(stage), nb * BN + 64 * i, k0, b);
+          }
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1u;
+          }
         }
       }
     }
@@ -264,84 +285,136 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   // ============================ consumer warpgroups ============================
   const int wg = warp >> 2;  // rows [64 wg, +64) of the tile
   const bool wg_leader = (threadIdx.x & 127) == 0;
-  float acc[BN / 2];
+  const int srow = (warp & 3) * 16 + (lane >> 2);  // this thread's first row within the warpgroup's 64
+  const int cq = 2 * (lane & 3);
+  const uint32_t stg = stg_base + wg * (2 * STG_BYTES);
+  uint32_t q = 0;  // sub-tiles this warpgroup has staged: selects the buffer
+  if (wg_leader && ep.tma_store) {
+    tma_prefetch_desc(&tmC);
+    if (SWIGLU) tma_prefetch_desc(&tmAux);
+  }
+
+  // One 64 x 64 bf16 sub-tile of the warpgroup's rows through smem: pair(j, h) is the bf16x2 at columns 8 j + cq, + 1
+  // of the thread's row srow + 8 h.  SWIZZLE_128B puts a row's 16-byte chunk c at c ^ (row & 7), so the 8 rows x 4
+  // quads of one warp write hit all 32 banks once.  The other buffer's store must have read it out before the barrier
+  // lets anyone write there; stores with a box wholly outside C (x >= x_end, y >= M) are skipped.
+  auto store_subtile = [&](const CUtensorMap* map, int x, int x_end, int y, int z, auto pair) {
+    const uint32_t buf = stg + (q & 1u) * STG_BYTES;
 #pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int h = 0; h < 2; ++h) {
+      const int row = srow + 8 * h;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const __nv_bfloat162 v = pair(j, h);
+        st_shared_b32(buf + row * 128 + ((j ^ (row & 7)) << 4) + 2 * cq, *reinterpret_cast<const uint32_t*>(&v));
+      }
+    }
+    fence_proxy_async_smem();
+    if (wg_leader) bulk_wait_read<0>();
+    named_bar_sync(1 + wg, 128);
+    if (wg_leader && x < x_end && y < M) {
+      tma_store_3d(map, buf, x, y, z);
+      bulk_commit();
+    }
+    ++q;
+  };
+
+  float acc[BN / 2];
   int stage = 0;
   uint32_t phase = 0;
-  int prev_stage = -1;
-  for (int kb = 0; kb < num_kb; ++kb) {
-    mbar_wait(full_bar(stage), phase);
-    const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES + wg * (64 * 128);
-    const uint32_t sb = smem_base + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES;
-    reg_fence(acc);
-    wgmma_fence();
+  for (int r = blockIdx.x; r < tiles; r += gridDim.x) {
+    const int b = r / tiles_per_batch;
+    int mb, nb;
+    tile_to_mn(r - b * tiles_per_batch, m_blocks, n_blocks, mb, nb);
+    const int m0 = mb * BM;
 #pragma unroll
-    for (int k = 0; k < BK / 16; ++k) {
-      const uint64_t adesc = A_MN ? make_smem_desc_sw128(sa + k * 2048, 64 * BK * 2, 1024)
-                                  : make_smem_desc_sw128(sa + k * 32, 0, 1024);
-      const uint64_t bdesc = B_MN ? make_smem_desc_sw128(sb + k * 2048, 64 * BK * 2, 1024)
-                                  : make_smem_desc_sw128(sb + k * 32, 0, 1024);
-      WgmmaSS<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>::mma(acc, adesc, bdesc, 1u);
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int prev_stage = -1;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(full_bar(stage), phase);
+      const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES + wg * (64 * 128);
+      const uint32_t sb = smem_base + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES;
+      reg_fence(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t adesc = A_MN ? make_smem_desc_sw128(sa + k * 2048, 64 * BK * 2, 1024)
+                                    : make_smem_desc_sw128(sa + k * 32, 0, 1024);
+        const uint64_t bdesc = B_MN ? make_smem_desc_sw128(sb + k * 2048, 64 * BK * 2, 1024)
+                                    : make_smem_desc_sw128(sb + k * 32, 0, 1024);
+        WgmmaSS<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>::mma(acc, adesc, bdesc, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage can be refilled
+      reg_fence(acc);
+      if (prev_stage >= 0 && wg_leader) mbar_arrive(empty_bar(prev_stage));
+      prev_stage = stage;
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1u;
+      }
     }
-    wgmma_commit();
-    wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage can be refilled
+    wgmma_wait<0>();
     reg_fence(acc);
-    if (prev_stage >= 0 && wg_leader) mbar_arrive(empty_bar(prev_stage));
-    prev_stage = stage;
-    if (++stage == STAGES) {
-      stage = 0;
-      phase ^= 1u;
-    }
-  }
-  wgmma_wait<0>();
-  reg_fence(acc);
+    if (wg_leader) mbar_arrive(empty_bar(prev_stage));  // the producer is already filling it with the next tile
 
-  // ============================ epilogue ============================
-  const int r_lo = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  const int cq = 2 * (lane & 3);
-  if constexpr (SWIGLU) {
-    // accumulator columns [0, BN/2) = gate, [BN/2, BN) = up of the same BN/2 features: write both pre-activations (saved
-    // for backward) and silu(gate) * up without a second pass over the [M, 2F] tensor
-    constexpr int JH = BN / 16;  // 8-column groups per half
-    const int F = N >> 1;
+    // ============================ epilogue ============================
+    const int y0 = m0 + wg * 64;
+    if constexpr (SWIGLU) {
+      // accumulator columns [0, BN/2) = gate, [BN/2, BN) = up of the same BN/2 features: write both pre-activations
+      // (saved for backward) and silu(gate) * up without a second pass over the [M, 2F] tensor
+      constexpr int JH = BN / 16;  // 8-column groups per half
+      const int F = N >> 1;
+      const int f0 = nb * (BN / 2);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = r_lo + 8 * h;
-      if (row >= M) continue;
-      bf16* gu = reinterpret_cast<bf16*>(ep.C) + static_cast<long long>(row) * ep.ldc;
-      bf16* ao = reinterpret_cast<bf16*>(ep.aux) + static_cast<long long>(row) * ep.ld_aux;
+      for (int s = 0; s < BN / 128; ++s)
+        store_subtile(&tmC, f0 + 64 * s, N, y0, 0, [&](int j, int h) {
+          return __floats2bfloat162_rn(acc[4 * (8 * s + j) + 2 * h], acc[4 * (8 * s + j) + 2 * h + 1]);
+        });
 #pragma unroll
-      for (int j = 0; j < JH; ++j) {
-        const int f = nb * (BN / 2) + 8 * j + cq;
-        // round to bf16 first: the separate kernels (and the reference) apply silu to the STORED bf16 pre-activations
-        const __nv_bfloat162 g2 = __floats2bfloat162_rn(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-        const __nv_bfloat162 u2 = __floats2bfloat162_rn(acc[4 * (j + JH) + 2 * h], acc[4 * (j + JH) + 2 * h + 1]);
-        const float2 g = __bfloat1622float2(g2), u = __bfloat1622float2(u2);
-        *reinterpret_cast<__nv_bfloat162*>(gu + f) = g2;
-        *reinterpret_cast<__nv_bfloat162*>(gu + F + f) = u2;
-        *reinterpret_cast<__nv_bfloat162*>(ao + f) = __floats2bfloat162_rn(silu(g.x) * u.x, silu(g.y) * u.y);
+      for (int s = 0; s < BN / 128; ++s)
+        store_subtile(&tmC, F + f0 + 64 * s, N, y0, 0, [&](int j, int h) {
+          return __floats2bfloat162_rn(acc[4 * (JH + 8 * s + j) + 2 * h], acc[4 * (JH + 8 * s + j) + 2 * h + 1]);
+        });
+#pragma unroll
+      for (int s = 0; s < BN / 128; ++s)
+        store_subtile(&tmAux, f0 + 64 * s, F, y0, 0, [&](int j, int h) {
+          // round to bf16 first: the separate kernels (and the reference) apply silu to the STORED pre-activations
+          const float2 g = __bfloat1622float2(
+              __floats2bfloat162_rn(acc[4 * (8 * s + j) + 2 * h], acc[4 * (8 * s + j) + 2 * h + 1]));
+          const float2 u = __bfloat1622float2(
+              __floats2bfloat162_rn(acc[4 * (JH + 8 * s + j) + 2 * h], acc[4 * (JH + 8 * s + j) + 2 * h + 1]));
+          return __floats2bfloat162_rn(silu(g.x) * u.x, silu(g.y) * u.y);
+        });
+    } else {
+      const int n0 = nb * BN;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = y0 + srow + 8 * h;
+        if (row >= M) continue;
+        const long long c_off = static_cast<long long>(b) * ep.bsc + static_cast<long long>(row) * ep.ldc;
+        const long long r_off = static_cast<long long>(b) * ep.bsr + static_cast<long long>(row) * ep.ldr;
+        if (ep.pair_ok) {
+          fuse_row<BN, ACT>(ep, c_off, r_off, n0 + cq, N, acc, h);
+          if (!ep.tma_store) store_row<BN>(ep, c_off, n0 + cq, N, acc, h);
+          continue;
+        }
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          if (n0 + 8 * j >= N) break;
+          epilogue_elems<ACT>(ep, c_off, r_off, n0 + 8 * j + cq, N, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
       }
-    }
-  } else {
-    const int n0 = nb * BN;
+      if (ep.tma_store) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = r_lo + 8 * h;
-      if (row >= M) continue;
-      const long long c_off = static_cast<long long>(b) * ep.bsc + static_cast<long long>(row) * ep.ldc;
-      const long long r_off = static_cast<long long>(b) * ep.bsr + static_cast<long long>(row) * ep.ldr;
-      if (ep.pair_ok) {
-        epilogue_row<BN, ACT>(ep, c_off, r_off, n0 + cq, N, acc, h);
-        continue;
-      }
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        if (n0 + 8 * j >= N) break;
-        epilogue_elems<ACT>(ep, c_off, r_off, n0 + 8 * j + cq, N, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        for (int s = 0; s < BN / 64; ++s)
+          store_subtile(&tmC, n0 + 64 * s, N, y0, b, [&](int j, int h) {
+            return __floats2bfloat162_rn(acc[4 * (8 * s + j) + 2 * h], acc[4 * (8 * s + j) + 2 * h + 1]);
+          });
       }
     }
   }
+  if (wg_leader) bulk_wait<0>();  // the CTA's smem must outlive the stores that read it
 }
 
 // ------------------------------------------------------------------------------------------
@@ -390,9 +463,14 @@ int make_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t inner, uint64
   return CB_OK;
 }
 
+// operand maps (A, B) and, for the TMA-store epilogue, the output maps (C, SwiGLU's second output); 64 x 64 store boxes
+struct GemmMaps {
+  CUtensorMap a, b, c, aux;
+};
+
 template <int BN, bool A_MN, bool B_MN, int ACT>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, int batch,
-                       const GemmEpilogue& ep, cudaStream_t stream) {
+static int launch_gemm(const GemmMaps& tm, int M, int N, int K, int batch, const GemmEpilogue& ep,
+                       cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
   auto kern = gemm_bf16_wgmma<BN, A_MN, B_MN, ACT>;
   static bool attr_set = false;
@@ -404,26 +482,27 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, in
   const int n_blocks = (ACT == ACT_SWIGLU_PAIR) ? (N / 2) / (BN / 2) : (N + BN - 1) / BN;
   const long long tiles = (long long)((M + BM - 1) / BM) * n_blocks * batch;
   CB_CHECK_ARG(tiles < (1LL << 31), "gemm: %lld tiles exceed the grid", tiles);
-  kern<<<(unsigned)tiles, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, M, N, K, ep);
+  const unsigned grid = (unsigned)std::min<long long>(tiles, device_sm_count());
+  kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tm.a, tm.b, tm.c, tm.aux, M, N, K, (int)tiles, ep);
   CB_CUDA_LAUNCH_CHECK("gemm_bf16_wgmma");
   return CB_OK;
 }
 
 template <int BN>
-static int dispatch_major(int a_mn, int b_mn, int act, const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N,
-                          int K, int batch, const GemmEpilogue& ep, cudaStream_t stream) {
+static int dispatch_major(int a_mn, int b_mn, int act, const GemmMaps& tm, int M, int N, int K, int batch,
+                          const GemmEpilogue& ep, cudaStream_t stream) {
   if (!a_mn && !b_mn) {
     switch (act) {
-      case 1: return launch_gemm<BN, false, false, 1>(tmA, tmB, M, N, K, batch, ep, stream);
-      case 2: return launch_gemm<BN, false, false, 2>(tmA, tmB, M, N, K, batch, ep, stream);
-      case 3: return launch_gemm<BN, false, false, 3>(tmA, tmB, M, N, K, batch, ep, stream);
-      case 4: return launch_gemm<BN, false, false, 4>(tmA, tmB, M, N, K, batch, ep, stream);
-      default: return launch_gemm<BN, false, false, 0>(tmA, tmB, M, N, K, batch, ep, stream);
+      case 1: return launch_gemm<BN, false, false, 1>(tm, M, N, K, batch, ep, stream);
+      case 2: return launch_gemm<BN, false, false, 2>(tm, M, N, K, batch, ep, stream);
+      case 3: return launch_gemm<BN, false, false, 3>(tm, M, N, K, batch, ep, stream);
+      case 4: return launch_gemm<BN, false, false, 4>(tm, M, N, K, batch, ep, stream);
+      default: return launch_gemm<BN, false, false, 0>(tm, M, N, K, batch, ep, stream);
     }
   }
-  if (!a_mn && b_mn) return launch_gemm<BN, false, true, 0>(tmA, tmB, M, N, K, batch, ep, stream);
-  if (a_mn && !b_mn) return launch_gemm<BN, true, false, 0>(tmA, tmB, M, N, K, batch, ep, stream);
-  return launch_gemm<BN, true, true, 0>(tmA, tmB, M, N, K, batch, ep, stream);
+  if (!a_mn && b_mn) return launch_gemm<BN, false, true, 0>(tm, M, N, K, batch, ep, stream);
+  if (a_mn && !b_mn) return launch_gemm<BN, true, false, 0>(tm, M, N, K, batch, ep, stream);
+  return launch_gemm<BN, true, true, 0>(tm, M, N, K, batch, ep, stream);
 }
 
 int gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int batch, long long lda,
@@ -448,13 +527,14 @@ int gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int ba
     else if (N > 128 && tiles(64) > 2LL * sms) bn = 128;
     else bn = 64;
   }
-  CUtensorMap tmA, tmB;
+  GemmMaps tm;
+  std::memset(&tm, 0, sizeof(tm));
   int rc;
-  if (!a_mn) rc = make_tmap_bf16_3d(&tmA, A, K, M, batch, lda, bsa, BM);
-  else       rc = make_tmap_bf16_3d(&tmA, A, M, K, batch, lda, bsa, BK);
+  if (!a_mn) rc = make_tmap_bf16_3d(&tm.a, A, K, M, batch, lda, bsa, BM);
+  else       rc = make_tmap_bf16_3d(&tm.a, A, M, K, batch, lda, bsa, BK);
   if (rc) return rc;
-  if (!b_mn) rc = make_tmap_bf16_3d(&tmB, B, K, N, batch, ldb, bsb, bn);
-  else       rc = make_tmap_bf16_3d(&tmB, B, N, K, batch, ldb, bsb, BK);
+  if (!b_mn) rc = make_tmap_bf16_3d(&tm.b, B, K, N, batch, ldb, bsb, bn);
+  else       rc = make_tmap_bf16_3d(&tm.b, B, N, K, batch, ldb, bsb, BK);
   if (rc) return rc;
   GemmEpilogue ep;
   ep.C = C; ep.ldc = ldc; ep.bsc = bsc;
@@ -463,7 +543,6 @@ int gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int ba
   ep.residual = static_cast<const bf16*>(residual);
   ep.ldr = ldr; ep.bsr = bsr;
   ep.alpha = alpha; ep.out_fp32 = out_fp32; ep.accumulate = accumulate;
-  ep.aux = nullptr; ep.ld_aux = 0;
   const unsigned calign = out_fp32 ? 7u : 3u;
   bool pair = (N % 2 == 0) && (ldc % 2 == 0) && (bsc % 2 == 0) && ((reinterpret_cast<uintptr_t>(C) & calign) == 0);
   if (residual)
@@ -471,10 +550,16 @@ int gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int ba
   if (bias) pair = pair && ((reinterpret_cast<uintptr_t>(bias) & 3u) == 0);
   if (colscale) pair = pair && ((reinterpret_cast<uintptr_t>(colscale) & 3u) == 0);
   ep.pair_ok = pair ? 1 : 0;
+  // bf16 C whose base and strides TMA can address takes the smem + TMA-store epilogue; fp32 C, and views at an odd
+  // element offset or stride, store from registers
+  const bool tma = pair && !out_fp32 && ((reinterpret_cast<uintptr_t>(C) & 15u) == 0) && ldc % 8 == 0 &&
+                   (batch == 1 || (bsc > 0 && bsc % 8 == 0));
+  if (tma && (rc = make_tmap_bf16_3d(&tm.c, C, N, M, batch, ldc, bsc, 64))) return rc;
+  ep.tma_store = tma ? 1 : 0;
   switch (bn) {
-    case 256: return dispatch_major<256>(a_mn, b_mn, act, tmA, tmB, M, N, K, batch, ep, stream);
-    case 128: return dispatch_major<128>(a_mn, b_mn, act, tmA, tmB, M, N, K, batch, ep, stream);
-    default:  return dispatch_major<64>(a_mn, b_mn, act, tmA, tmB, M, N, K, batch, ep, stream);
+    case 256: return dispatch_major<256>(a_mn, b_mn, act, tm, M, N, K, batch, ep, stream);
+    case 128: return dispatch_major<128>(a_mn, b_mn, act, tm, M, N, K, batch, ep, stream);
+    default:  return dispatch_major<64>(a_mn, b_mn, act, tm, M, N, K, batch, ep, stream);
   }
 }
 
@@ -492,16 +577,17 @@ int gemm_swiglu_bf16(const void* A, const void* W, void* gu_out, void* act_out, 
   // 128 gate + 128 up features per tile: the same 128 x 256 tile and operand traffic per FLOP as the generic BN = 256
   // kernel (a 64 + 64 tile reads 32 KB of operands per 64-deep k-block for half the FLOPs of a 48 KB 128 x 256 k-block)
   constexpr int BN = 256;
-  CUtensorMap tmA, tmB;
+  GemmMaps tm;
   int rc;
-  if ((rc = make_tmap_bf16_3d(&tmA, A, K, M, 1, lda, 0, BM))) return rc;
-  if ((rc = make_tmap_bf16_3d(&tmB, W, K, N, 1, ldw, 0, BN / 2))) return rc;
+  if ((rc = make_tmap_bf16_3d(&tm.a, A, K, M, 1, lda, 0, BM))) return rc;
+  if ((rc = make_tmap_bf16_3d(&tm.b, W, K, N, 1, ldw, 0, BN / 2))) return rc;
+  if ((rc = make_tmap_bf16_3d(&tm.c, gu_out, N, M, 1, ld_gu, 0, 64))) return rc;
+  if ((rc = make_tmap_bf16_3d(&tm.aux, act_out, F, M, 1, ld_act, 0, 64))) return rc;
   GemmEpilogue ep;
   ep.C = gu_out; ep.ldc = ld_gu; ep.bsc = 0;
   ep.bias = nullptr; ep.colscale = nullptr; ep.residual = nullptr; ep.ldr = 0; ep.bsr = 0;
-  ep.alpha = 1.0f; ep.out_fp32 = 0; ep.accumulate = 0; ep.pair_ok = 1;
-  ep.aux = act_out; ep.ld_aux = ld_act;
-  return launch_gemm<BN, false, false, ACT_SWIGLU_PAIR>(tmA, tmB, M, N, K, 1, ep, stream);
+  ep.alpha = 1.0f; ep.out_fp32 = 0; ep.accumulate = 0; ep.pair_ok = 1; ep.tma_store = 1;
+  return launch_gemm<BN, false, false, ACT_SWIGLU_PAIR>(tm, M, N, K, 1, ep, stream);
 }
 
 }  // namespace cb

@@ -71,7 +71,7 @@ def step_shapes(config):
         ("dec.qkv fwd", fwd, g(R, QKV, H)),
         ("dec.o fwd +res", fwd, g(R, H, H, residual=True)),
         ("dec.gate_up+swiglu fwd", fwd, g(R, 2 * I, H, swiglu=True)),
-        ("dec.down fwd +res", fwd, g(R, H, I, residual=True)),
+        ("dec.down fwd +res", L, g(R, H, I, residual=True)),   # the recompute stops before the down projection
         ("dec.down dX", L, g(R, I, H, b_mn=True)),
         ("dec.gate_up dX", L, g(R, H, 2 * I, b_mn=True)),
         ("dec.o dX", L, g(R, H, H, b_mn=True)),
@@ -85,9 +85,13 @@ def step_shapes(config):
         ("lm_head dW +=", n_chunks, g(V, H, chunk, a_mn=True, b_mn=True, acc=True)),
     ]
     if "clip-convnext-XXL" in c["towers"]:
-        cn_rows = B * (c["res"][c["towers"].index("clip-convnext-XXL")] // 16) ** 2   # stage 3: stride 16, 1536 ch, 30 blocks
-        rows += [("convnext s3 fc1 gelu", 30, g(cn_rows, 4 * 1536, 1536, act="gelu", bias=True)),
-                 ("convnext s3 fc2 ls+res", 30, g(cn_rows, 1536, 4 * 1536, bias=True, colscale=True, residual=True))]
+        res = c["res"][c["towers"].index("clip-convnext-XXL")]
+        # stages 1-3: stride 4 / 8 / 16, 384 / 768 / 1536 channels, 3 / 4 / 30 blocks (stage 4 is small)
+        for st, stride, C, blocks in ((1, 4, 384, 3), (2, 8, 768, 4), (3, 16, 1536, 30)):
+            cn_rows = B * (res // stride) ** 2
+            rows += [(f"convnext s{st} fc1 gelu", blocks, g(cn_rows, 4 * C, C, act="gelu", bias=True)),
+                     (f"convnext s{st} fc2 ls+res", blocks,
+                      g(cn_rows, C, 4 * C, bias=True, colscale=True, residual=True))]
     if any("siglip" in t for t in c["towers"]):
         rows += [("siglip fc1 gelu", 27, g(B * 729, 4304, 1152, act="gelu", bias=True))]
     if any("clip-vit-large" in t for t in c["towers"]):
