@@ -54,10 +54,10 @@ long long norm_bwd_workspace_floats(long long, int);
 int attn_fwd_launch(const void*, const void*, const void*, void*, float*, const void*, int, int, int, int, int, int,
                     long long, long long, long long, long long, long long, long long, long long, long long, float, int,
                     cudaStream_t);
-int attn_bwd_launch(const void*, const void*, const void*, const void*, const void*, const float*, float*, float*, void*,
+int attn_bwd_launch(const void*, const void*, const void*, const void*, const void*, const float*, float*, void*, void*,
                     void*, const void*, int, int, int, int, int, int, long long, long long, long long, long long,
                     long long, long long, long long, long long, long long, long long, long long, long long, long long,
-                    long long, float, int, cudaStream_t);
+                    long long, long long, long long, float, int, cudaStream_t);
 int act_fwd_launch(const void*, void*, long long, int, cudaStream_t);
 int act_bwd_launch(const void*, const void*, void*, long long, int, cudaStream_t);
 int swiglu_fwd_launch(const void*, const void*, void*, long long, int, long long, long long, cudaStream_t);
@@ -167,13 +167,13 @@ int cb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse
                              o_ss, scale, causal, ST(stream));
 }
 int cb_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
-                float* delta, float* dq_acc, void* dk, void* dv, const void* kmask, int B, int nh, int nkv, int Sq,
+                float* delta, void* dq, void* dk, void* dv, const void* kmask, int B, int nh, int nkv, int Sq,
                 int Skv, int hd, int64_t q_bs, int64_t q_ss, int64_t k_bs, int64_t k_ss, int64_t v_bs, int64_t v_ss,
-                int64_t o_bs, int64_t o_ss, int64_t do_bs, int64_t do_ss, int64_t dk_bs, int64_t dk_ss,
-                int64_t dv_bs, int64_t dv_ss, float scale, int causal, void* stream) {
-  return cb::attn_bwd_launch(q, k, v, o, d_o, lse, delta, dq_acc, dk, dv, kmask, B, nh, nkv, Sq, Skv, hd, q_bs, q_ss,
-                             k_bs, k_ss, v_bs, v_ss, o_bs, o_ss, do_bs, do_ss, dk_bs, dk_ss, dv_bs, dv_ss, scale, causal,
-                             ST(stream));
+                int64_t o_bs, int64_t o_ss, int64_t do_bs, int64_t do_ss, int64_t dq_bs, int64_t dq_ss,
+                int64_t dk_bs, int64_t dk_ss, int64_t dv_bs, int64_t dv_ss, float scale, int causal, void* stream) {
+  return cb::attn_bwd_launch(q, k, v, o, d_o, lse, delta, dq, dk, dv, kmask, B, nh, nkv, Sq, Skv, hd, q_bs, q_ss,
+                             k_bs, k_ss, v_bs, v_ss, o_bs, o_ss, do_bs, do_ss, dq_bs, dq_ss, dk_bs, dk_ss, dv_bs, dv_ss,
+                             scale, causal, ST(stream));
 }
 int cb_act_fwd(const void* x, void* y, int64_t n, int act, void* stream) {
   return cb::act_fwd_launch(x, y, n, act, ST(stream));

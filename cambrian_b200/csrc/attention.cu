@@ -15,12 +15,17 @@
 //              A operand of O += P_j V_j (wgmma with A from registers, V read MN-major from shared memory).
 // Backward, two kernels so that every output element has exactly one writer (no atomics: bit-identical run to run):
 //   dK / dV: one CTA = 128 keys of one KV head, two warpgroups of 64 keys, looping over the query heads of the GQA group
-//     and the 64-row query tiles: S^T = K Q^T and dP^T = V dO^T in registers; P^T and dS^T are re-packed in registers as
-//     the A operands of dV += P^T dO and dK += dS^T Q.
+//     and the 64-row query tiles, which a producer warp streams (with their lse / delta slices) through an mbarrier
+//     ring: S^T = K Q^T and dP^T = V dO^T in registers; P^T and dS^T are re-packed in registers as the A operands of
+//     dV += P^T dO and dK += dS^T Q.
 //   dQ: one CTA = 128 queries of one head (same layout as the forward), looping over 64-key tiles: S = Q K^T and
-//     dP = dO V^T in registers, dS re-packed as the A operand of dQ += dS K; dQ is stored once per element.
+//     dP = dO V^T in registers, dS re-packed as the A operand of dQ += dS K; dQ x scale is stored once per element, as
+//     bf16, into the caller's view.
+// Tiles that every (query, key) pair of a warp can see skip the per-element masking; grids are 1-D, heaviest causal
+// tiles first.
 #include "common.cuh"
 #include <cudaTypedefs.h>
+#include <type_traits>
 
 namespace cb {
 
@@ -38,11 +43,42 @@ struct AttnParams {
   float scale_log2;      // softmax scale * log2(e)
 };
 
+// true iff every key of [k0, k0 + N) is set in the key mask (the caller checks k0 + N <= Skv): N / 32 bytes per lane in
+// one load where aligned, and a warp vote, so the result is warp-uniform.  Tiles that pass skip the per-element masking.
+template <int N>
+__device__ __forceinline__ bool keys_all_valid(const uint8_t* km, int k0) {
+  constexpr int PER = N / 32;
+  static_assert(PER == 2 || PER == 4, "64- or 128-key tiles");
+  const uint8_t* kp = km + k0 + PER * (threadIdx.x & 31);
+  uint32_t w = 0;
+  if (!(reinterpret_cast<uintptr_t>(kp) & (PER - 1))) {
+    w = PER == 4 ? *reinterpret_cast<const uint32_t*>(kp) : *reinterpret_cast<const uint16_t*>(kp);
+  } else {
+#pragma unroll
+    for (int i = 0; i < PER; ++i) w |= (uint32_t)kp[i] << (8 * i);
+  }
+  bool ok = true;
+#pragma unroll
+  for (int i = 0; i < PER; ++i) ok = ok && ((w >> (8 * i)) & 0xffu);
+  return __all_sync(0xffffffffu, ok);
+}
+
+// Grids are 1-D with the tile index slowest, so the first wave holds the heaviest causal tiles of every (head, batch)
+// and the light ones fill the tail.
+struct TileIdx {
+  int t, h, b;
+};
+__device__ __forceinline__ TileIdx tile_index(int heads, int B) {
+  const int hb = heads * B;
+  const int rem = (int)blockIdx.x % hb;
+  return {(int)blockIdx.x / hb, rem % heads, rem / heads};
+}
+
 template <int HDP>
 struct FwdCfg {
   static constexpr int ATOMS = (HDP + 63) / 64;
   static constexpr int TILE = ATOMS * 16384;         // one [128 x hd] operand tile, 64-column SWIZZLE_128B atoms
-  static constexpr int STAGES = (HDP <= 64) ? 3 : 2;
+  static constexpr int STAGES = 3;                   // hd 128: 32 KB Q + 3 x 64 KB K / V
   static constexpr int SMEM = TILE * (1 + 2 * STAGES) + 1024 + 256;
 };
 
@@ -65,8 +101,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q_tiles = (p.Sq + 127) / 128;
-  const int qt = q_tiles - 1 - (int)blockIdx.x;  // heavy (late) causal tiles first
-  const int h = blockIdx.y, b = blockIdx.z;
+  const TileIdx ti = tile_index(p.nh, p.B);
+  const int qt = q_tiles - 1 - ti.t;  // heavy (late) causal tiles first
+  const int h = ti.h, b = ti.b;
   const int hk = h / (p.nh / p.nkv);
   const int q0 = qt * 128;
   const int kv_tiles_all = (p.Skv + 127) / 128;
@@ -143,10 +180,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
                               make_smem_desc_sw128(kb + off, 0, 1024), kk ? 1u : 0u);
     }
     wgmma_commit();
+    // masking (keys past Skv, past the diagonal, padded keys) -> -inf; scores into the log2 domain.  A tile inside Skv,
+    // below the diagonal for all 64 rows of the warpgroup, whose keys are all valid keeps every score as it is.
+    bool full_tile = k0 + 128 <= p.Skv && (!p.causal || k0 + 127 <= q0 + wg * 64 + coff);
+    if (full_tile && km) full_tile = keys_all_valid<128>(km, k0);
     wgmma_wait<0>();
     reg_fence(s);
-    // masking (keys past Skv, past the diagonal, padded keys) -> -inf; scores into the log2 domain
-    const bool full_tile = !km && k0 + 128 <= p.Skv && (!p.causal || k0 + 127 <= q0 + wg * 64 + coff);
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int jj = 0; jj < 16; ++jj) {
@@ -264,10 +303,10 @@ __global__ void attn_delta_kernel(const bf16* __restrict__ o, const bf16* __rest
 }
 
 struct AttnBwdParams {
-  float* dq_acc;            // [B, Sq, nh, hd] fp32: receives dS K (unscaled), every element written once
-  bf16* dk;                 // (b, s, kv head, d) with strides below
+  bf16* dq;                 // (b, s, head, d) with strides below: dS K x softmax scale, every element written once
+  bf16* dk;                 // (b, s, kv head, d)
   bf16* dv;
-  long long dk_bs, dk_ss, dv_bs, dv_ss;
+  long long dq_bs, dq_ss, dk_bs, dk_ss, dv_bs, dv_ss;
   const float* lse;         // [B, nh, Sq] log2 domain
   const float* delta;       // [B, nh, Sq]
   const uint8_t* kmask;
@@ -280,26 +319,35 @@ struct BwdCfg {
   static constexpr int ATOMS = HDP / 64;
   static constexpr int KTILE = ATOMS * 16384;  // [128 keys x hd]
   static constexpr int QTILE = ATOMS * 8192;   // [64 queries x hd]
-  static constexpr int SMEM = 2 * KTILE + 4 * QTILE + 1024 + 256;
+  static constexpr int STAGES = 4;             // Q / dO ring; each stage also holds the tile's lse[64] and delta[64]
+  static constexpr int SMEM = 2 * KTILE + 2 * STAGES * QTILE + STAGES * 512 + 1024 + 256;
 };
 
+// 384 threads: warpgroups 0-1 consume (dK and dV alone hold HDP fp32 per thread), warp 8 of warpgroup 2 produces.
+// Registers are allocated per 4 warps, so a 288-thread CTA would cap every thread at 168; setmaxnreg moves the
+// producer warpgroup's share to the consumers instead (128 x 24 + 256 x 240 <= 64 K).
 template <int HDP>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(384, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, AttnBwdParams p) {
   using Cfg = BwdCfg<HDP>;
+  constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sK = base;
   const uint32_t sV = sK + Cfg::KTILE;
-  const uint32_t sQ = sV + Cfg::KTILE;       // 2 stages
-  const uint32_t sdO = sQ + 2 * Cfg::QTILE;  // 2 stages
-  const uint32_t bars = sdO + 2 * Cfg::QTILE;
+  const uint32_t sQ = sV + Cfg::KTILE;
+  const uint32_t sdO = sQ + STAGES * Cfg::QTILE;
+  const uint32_t sLD = sdO + STAGES * Cfg::QTILE;
+  const uint32_t bars = sLD + STAGES * 512;
   const uint32_t kv_full = bars;
   auto qd_full = [&](int s) { return bars + 8u * (1 + s); };
+  auto qd_empty = [&](int s) { return bars + 8u * (1 + STAGES + s); };
+  float* ld_stage = reinterpret_cast<float*>(smem_raw + (sLD - smem_u32(smem_raw)));  // [STAGES][lse 64 | delta 64]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int jt = blockIdx.x, g = blockIdx.y, b = blockIdx.z;
+  const TileIdx ti = tile_index(p.nkv, p.B);
+  const int jt = ti.t, g = ti.h, b = ti.b;  // key tile 0 is seen by every query: heavy tiles first
   const int G = p.nh / p.nkv;
   const int k0 = jt * 128;
   const int q_tiles = (p.Sq + 63) / 64;
@@ -313,56 +361,84 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int n_i = q_tiles > i_begin ? q_tiles - i_begin : 0;
   const int n_iter = n_i * G;
 
-  auto load_qd = [&](int it) {
-    const int st = it & 1;
-    const int h = g * G + it / n_i;
-    const int qi0 = (i_begin + it % n_i) * 64;
-    mbar_arrive_expect_tx(qd_full(st), 2 * Cfg::QTILE);
-#pragma unroll
-    for (int a = 0; a < Cfg::ATOMS; ++a) {
-      tma_load_4d(sQ + st * Cfg::QTILE + a * 8192, &tmQ, qd_full(st), a * 64, h, qi0, b);
-      tma_load_4d(sdO + st * Cfg::QTILE + a * 8192, &tmdO, qd_full(st), a * 64, h, qi0, b);
-    }
-  };
-  if (threadIdx.x == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     tma_prefetch_desc(&tmdO);
     mbar_init(kv_full, 1);
-    mbar_init(qd_full(0), 1);
-    mbar_init(qd_full(1), 1);
-    mbar_fence_init();
-    mbar_arrive_expect_tx(kv_full, 2 * Cfg::KTILE);
-#pragma unroll
-    for (int a = 0; a < Cfg::ATOMS; ++a) {
-      tma_load_4d(sK + a * 16384, &tmK, kv_full, a * 64, g, k0, b);
-      tma_load_4d(sV + a * 16384, &tmV, kv_full, a * 64, g, k0, b);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(qd_full(s), 1 + 32);  // the TMA transaction arrive + one per producer lane after its lse / delta stores
+      mbar_init(qd_empty(s), 8);      // one arrive per consumer warp
     }
-    if (n_iter > 0) load_qd(0);
-    if (n_iter > 1) load_qd(1);
+    mbar_fence_init();
   }
   __syncthreads();
 
+  if (warp >= 8) {
+    // ================================ producer warp ================================
+    setmaxnreg_dec<24>();
+    if (warp > 8) return;
+    if (lane == 0) {
+      mbar_arrive_expect_tx(kv_full, 2 * Cfg::KTILE);
+#pragma unroll
+      for (int a = 0; a < Cfg::ATOMS; ++a) {
+        tma_load_4d(sK + a * 16384, &tmK, kv_full, a * 64, g, k0, b);
+        tma_load_4d(sV + a * 16384, &tmV, kv_full, a * 64, g, k0, b);
+      }
+    }
+    int st = 0;
+    uint32_t ph = 0;
+    for (int it = 0; it < n_iter; ++it) {
+      const int h = g * G + it / n_i;
+      const int qi0 = (i_begin + it % n_i) * 64;
+      mbar_wait(qd_empty(st), ph ^ 1u);
+      if (lane == 0) {
+        mbar_arrive_expect_tx(qd_full(st), 2 * Cfg::QTILE);
+#pragma unroll
+        for (int a = 0; a < Cfg::ATOMS; ++a) {
+          tma_load_4d(sQ + st * Cfg::QTILE + a * 8192, &tmQ, qd_full(st), a * 64, h, qi0, b);
+          tma_load_4d(sdO + st * Cfg::QTILE + a * 8192, &tmdO, qd_full(st), a * 64, h, qi0, b);
+        }
+      }
+      const float* lse = p.lse + ((long long)b * p.nh + h) * p.Sq;
+      const float* dlt = p.delta + ((long long)b * p.nh + h) * p.Sq;
+      float* ld = ld_stage + st * 128;
+#pragma unroll
+      for (int i = lane; i < 64; i += 32) {
+        const int qi = qi0 + i;
+        ld[i] = qi < p.Sq ? __ldg(lse + qi) : 0.f;
+        ld[64 + i] = qi < p.Sq ? __ldg(dlt + qi) : 0.f;
+      }
+      mbar_arrive(qd_full(st));
+      if (++st == STAGES) { st = 0; ph ^= 1u; }
+    }
+    return;
+  }
+
+  // ================================ consumer warpgroups ================================
+  setmaxnreg_inc<240>();
   const int wg = warp >> 2;
   const int kr = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's key rows kr, kr + 8 (S^T, dK, dV)
   const int cq = 2 * (lane & 3);
+  const int wk0 = k0 + wg * 64 + (warp & 3) * 16;          // this warp's 16 key rows start here
   bool key_ok[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int kidx = k0 + kr + 8 * r;
     key_ok[r] = kidx < p.Skv && (!p.kmask || p.kmask[(size_t)b * p.Skv + kidx]);
   }
+  const bool warp_keys_ok = __all_sync(0xffffffffu, key_ok[0] && key_ok[1]);
   float dv[HDP / 2], dk[HDP / 2];
 #pragma unroll
   for (int i = 0; i < HDP / 2; ++i) dv[i] = dk[i] = 0.f;
   mbar_wait(kv_full, 0);
+  int st = 0;
+  uint32_t ph = 0;
   for (int it = 0; it < n_iter; ++it) {
-    const int st = it & 1;
-    const int h = g * G + it / n_i;
     const int qi0 = (i_begin + it % n_i) * 64;
     const uint32_t qb = sQ + st * Cfg::QTILE, dob = sdO + st * Cfg::QTILE;
-    mbar_wait(qd_full(st), (it >> 1) & 1);
+    mbar_wait(qd_full(st), ph);
     float sT[32], dpT[32];
     wgmma_fence();
 #pragma unroll
@@ -378,36 +454,45 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
                              make_smem_desc_sw128(dob + qoff, 0, 1024), kk ? 1u : 0u);
     }
     wgmma_commit();
+    // every (key, query) pair of the tile is visible to this warp: all 64 queries exist, the warp's 16 keys are valid
+    // and none lies past the diagonal of the tile's first query
+    const bool full = warp_keys_ok && qi0 + 64 <= p.Sq && (!p.causal || wk0 + 15 <= qi0 + coff);
+    const float* ld = ld_stage + st * 128;
     wgmma_wait<0>();
     reg_fence(sT);
     reg_fence(dpT);
     // P^T = exp2(S^T * scale - lse) on visible (key, query) pairs, dS^T = P^T * (dP^T - delta): bf16 A fragments of
     // dV += P^T dO and dK += dS^T Q
-    const float* lse = p.lse + ((long long)b * p.nh + h) * p.Sq;
-    const float* dlt = p.delta + ((long long)b * p.nh + h) * p.Sq;
     uint32_t pa[4][4], da[4][4];
+    auto grads = [&](auto full_tile) {
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
-      float pv[4], dsv[4];
+      for (int jj = 0; jj < 8; ++jj) {
+        float pv[4], dsv[4];
 #pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        const int qi = qi0 + 8 * jj + cq + c;
-        const bool q_ok = qi < p.Sq;
-        const float L = q_ok ? __ldg(lse + qi) : 0.f, D = q_ok ? __ldg(dlt + qi) : 0.f;
+        for (int c = 0; c < 2; ++c) {
+          const int qc = 8 * jj + cq + c;
+          const float L = ld[qc], D = ld[64 + qc];
 #pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          const int e = 2 * r + c;
-          const bool vis = q_ok && key_ok[r] && (!p.causal || k0 + kr + 8 * r <= qi + coff);
-          const float pe = vis ? fast_exp2(fmaf(sT[4 * jj + e], p.scale_log2, -L)) : 0.f;
-          pv[e] = pe;
-          dsv[e] = pe * (dpT[4 * jj + e] - D);
+          for (int r = 0; r < 2; ++r) {
+            const int e = 2 * r + c;
+            bool vis = true;
+            if (!decltype(full_tile)::value)
+              vis = qi0 + qc < p.Sq && key_ok[r] && (!p.causal || k0 + kr + 8 * r <= qi0 + qc + coff);
+            const float pe = vis ? fast_exp2(fmaf(sT[4 * jj + e], p.scale_log2, -L)) : 0.f;
+            pv[e] = pe;
+            dsv[e] = pe * (dpT[4 * jj + e] - D);
+          }
         }
+        pa[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(pv[0], pv[1]);
+        pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(pv[2], pv[3]);
+        da[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(dsv[0], dsv[1]);
+        da[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(dsv[2], dsv[3]);
       }
-      pa[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(pv[0], pv[1]);
-      pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(pv[2], pv[3]);
-      da[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(dsv[0], dsv[1]);
-      da[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(dsv[2], dsv[3]);
-    }
+    };
+    if (full)
+      grads(std::true_type());
+    else
+      grads(std::false_type());
     reg_fence(dv);
     reg_fence(dk);
     wgmma_fence();
@@ -420,8 +505,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     wgmma_wait<0>();
     reg_fence(dv);
     reg_fence(dk);
-    __syncthreads();  // this iteration's Q / dO stage is no longer read by either warpgroup
-    if (threadIdx.x == 0 && it + 2 < n_iter) load_qd(it + 2);
+    if (lane == 0) mbar_arrive(qd_empty(st));  // this warp no longer reads the stage (wgmma operands, lse / delta)
+    if (++st == STAGES) { st = 0; ph ^= 1u; }
   }
   // ---- epilogue: dK (x softmax scale), dV -> bf16 (zeros for keys no query sees)
 #pragma unroll
@@ -445,7 +530,7 @@ struct DqCfg {
   static constexpr int ATOMS = HDP / 64;
   static constexpr int QTILE = ATOMS * 16384;  // [128 queries x hd]
   static constexpr int KTILE = ATOMS * 8192;   // [64 keys x hd]
-  static constexpr int STAGES = 2;
+  static constexpr int STAGES = 4;
   static constexpr int SMEM = 2 * QTILE + 2 * STAGES * KTILE + 1024 + 256;
 };
 
@@ -468,8 +553,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q_tiles = (p.Sq + 127) / 128;
-  const int qt = q_tiles - 1 - (int)blockIdx.x;  // heavy (late) causal tiles first
-  const int h = blockIdx.y, b = blockIdx.z;
+  const TileIdx ti = tile_index(p.nh, p.B);
+  const int qt = q_tiles - 1 - ti.t;  // heavy (late) causal tiles first
+  const int h = ti.h, b = ti.b;
   const int hk = h / (p.nh / p.nkv);
   const int q0 = qt * 128;
   const int coff = p.Skv - p.Sq;
@@ -521,6 +607,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const bool wg_leader = (threadIdx.x & 127) == 0;
   const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's query rows: rloc and rloc + 8
   const int cq = 2 * (lane & 3);
+  const int wq0 = q0 + wg * 64 + (warp & 3) * 16;             // this warp's 16 query rows start here
   const uint8_t* km = p.kmask ? p.kmask + (size_t)b * p.Skv : nullptr;
   const float* lse = p.lse + ((long long)b * p.nh + h) * p.Sq;
   const float* dlt = p.delta + ((long long)b * p.nh + h) * p.Sq;
@@ -557,24 +644,36 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
                              kk ? 1u : 0u);
     }
     wgmma_commit();
+    // every (query, key) pair of the tile is visible to this warp: the 64 keys lie inside Skv, at or before the
+    // diagonal of the warp's first query, and are all valid; the warp's 16 queries exist
+    bool full = k0 + 64 <= p.Skv && wq0 + 16 <= p.Sq && (!p.causal || k0 + 63 <= wq0 + coff);
+    if (full && km) full = keys_all_valid<64>(km, k0);
     wgmma_wait<0>();
     reg_fence(s);
     reg_fence(dp);
     // dS = P * (dP - delta), P = exp2(S * scale - lse) on visible (query, key) pairs: bf16 A fragments of dQ += dS K
     uint32_t da[4][4];
+    auto grads = [&](auto full_tile) {
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
-      float dsv[4];
+      for (int jj = 0; jj < 8; ++jj) {
+        float dsv[4];
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int r = e >> 1, key = k0 + 8 * jj + cq + (e & 1);
-        const bool vis = qi[r] < p.Sq && key < p.Skv && (!p.causal || key <= qi[r] + coff) && (!km || km[key]);
-        const float pe = vis ? fast_exp2(fmaf(s[4 * jj + e], p.scale_log2, -L[r])) : 0.f;
-        dsv[e] = pe * (dp[4 * jj + e] - D[r]);
+        for (int e = 0; e < 4; ++e) {
+          const int r = e >> 1, key = k0 + 8 * jj + cq + (e & 1);
+          bool vis = true;
+          if (!decltype(full_tile)::value)
+            vis = qi[r] < p.Sq && key < p.Skv && (!p.causal || key <= qi[r] + coff) && (!km || km[key]);
+          const float pe = vis ? fast_exp2(fmaf(s[4 * jj + e], p.scale_log2, -L[r])) : 0.f;
+          dsv[e] = pe * (dp[4 * jj + e] - D[r]);
+        }
+        da[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(dsv[0], dsv[1]);
+        da[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(dsv[2], dsv[3]);
       }
-      da[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(dsv[0], dsv[1]);
-      da[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(dsv[2], dsv[3]);
-    }
+    };
+    if (full)
+      grads(std::true_type());
+    else
+      grads(std::false_type());
     reg_fence(dq);
     wgmma_fence();
 #pragma unroll
@@ -586,13 +685,15 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     if (wg_leader) mbar_arrive(kv_empty(st));
     if (++st == STAGES) { st = 0; ph ^= 1u; }
   }
+  // ---- epilogue: dQ x softmax scale in fp32, rounded once to bf16 (the caller's view may be a packed dQKV buffer)
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     if (qi[r] >= p.Sq) continue;
-    float* dqp = p.dq_acc + (((long long)b * p.Sq + qi[r]) * p.nh + h) * p.hd;
+    bf16* dqp = p.dq + (long long)b * p.dq_bs + (long long)qi[r] * p.dq_ss + (long long)h * p.hd;
 #pragma unroll
     for (int jj = 0; jj < HDP / 8; ++jj)
-      *reinterpret_cast<float2*>(dqp + 8 * jj + cq) = make_float2(dq[4 * jj + 2 * r], dq[4 * jj + 2 * r + 1]);
+      *reinterpret_cast<__nv_bfloat162*>(dqp + 8 * jj + cq) =
+          __floats2bfloat162_rn(dq[4 * jj + 2 * r] * p.scale, dq[4 * jj + 2 * r + 1] * p.scale);
   }
 }
 
@@ -648,8 +749,7 @@ static int launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtens
     if (e != cudaSuccess) return set_error(CB_ERR_CUDA, "attn fwd smem attr: %s", cudaGetErrorString(e));
     attr = true;
   }
-  dim3 grid((p.Sq + 127) / 128, p.nh, p.B);
-  kern<<<grid, 288, Cfg::SMEM, st>>>(tq, tk, tv, p);
+  kern<<<(p.Sq + 127) / 128 * p.nh * p.B, 288, Cfg::SMEM, st>>>(tq, tk, tv, p);
   CB_CUDA_LAUNCH_CHECK("attn_fwd");
   return CB_OK;
 }
@@ -690,8 +790,7 @@ static int launch_bwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtens
     if (e != cudaSuccess) return set_error(CB_ERR_CUDA, "attn bwd smem attr: %s", cudaGetErrorString(e));
     attr = true;
   }
-  dim3 grid((p.Skv + 127) / 128, p.nkv, p.B);
-  kern<<<grid, 256, Cfg::SMEM, st>>>(tq, tk, tv, tdo, p);
+  kern<<<(p.Skv + 127) / 128 * p.nkv * p.B, 384, Cfg::SMEM, st>>>(tq, tk, tv, tdo, p);
   CB_CUDA_LAUNCH_CHECK("attn_bwd");
   return CB_OK;
 }
@@ -707,22 +806,23 @@ static int launch_bwd_dq(const CUtensorMap& tq, const CUtensorMap& tk, const CUt
     if (e != cudaSuccess) return set_error(CB_ERR_CUDA, "attn bwd dq smem attr: %s", cudaGetErrorString(e));
     attr = true;
   }
-  dim3 grid((p.Sq + 127) / 128, p.nh, p.B);
-  kern<<<grid, 288, Cfg::SMEM, st>>>(tq, tk, tv, tdo, p);
+  kern<<<(p.Sq + 127) / 128 * p.nh * p.B, 288, Cfg::SMEM, st>>>(tq, tk, tv, tdo, p);
   CB_CUDA_LAUNCH_CHECK("attn_bwd_dq");
   return CB_OK;
 }
 
 int attn_bwd_launch(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
-                    float* delta, float* dq_acc, void* dk, void* dv, const void* kmask, int B, int nh, int nkv,
+                    float* delta, void* dq, void* dk, void* dv, const void* kmask, int B, int nh, int nkv,
                     int Sq, int Skv, int hd, long long q_bs, long long q_ss, long long k_bs, long long k_ss,
                     long long v_bs, long long v_ss, long long o_bs, long long o_ss, long long do_bs, long long do_ss,
-                    long long dk_bs, long long dk_ss, long long dv_bs, long long dv_ss, float scale, int causal,
-                    cudaStream_t st) {
+                    long long dq_bs, long long dq_ss, long long dk_bs, long long dk_ss, long long dv_bs,
+                    long long dv_ss, float scale, int causal, cudaStream_t st) {
   CB_CHECK_ARG(B > 0 && nh > 0 && nkv > 0 && Sq > 0 && Skv > 0, "attention bwd: empty problem");
   CB_CHECK_ARG(nh % nkv == 0, "attention bwd: nh=%d not a multiple of nkv=%d", nh, nkv);
   CB_CHECK_ARG(hd == 64 || hd == 128, "attention bwd: head_dim=%d unsupported (64 or 128)", hd);
-  CB_CHECK_ARG(lse && delta && dq_acc, "attention bwd: lse / delta / dq_acc buffers are required");
+  CB_CHECK_ARG(lse && delta && dq && dk && dv, "attention bwd: lse / delta / dq / dk / dv buffers are required");
+  CB_CHECK_ARG(!(reinterpret_cast<uintptr_t>(dq) & 3u) && dq_bs % 2 == 0 && dq_ss % 2 == 0,
+               "attention bwd: dq must be 4-byte aligned with even strides");
   {
     const long long warps = ((long long)B * Sq * nh + (256 / hd) - 1) / (256 / hd);   // 32 / (hd / 8) heads per warp
     attn_delta_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>((const bf16*)o, (const bf16*)d_o, delta, B,
@@ -736,12 +836,11 @@ int attn_bwd_launch(const void* q, const void* k, const void* v, const void* o, 
   if ((rc = make_tmap_bf16_4d(&tv, v, hd, nkv, Skv, B, hd, v_ss, v_bs, 128))) return rc;
   if ((rc = make_tmap_bf16_4d(&tdo, d_o, hd, nh, Sq, B, hd, do_ss, do_bs, 64))) return rc;
   AttnBwdParams p;
-  p.dq_acc = dq_acc; p.dk = (bf16*)dk; p.dv = (bf16*)dv;
-  p.dk_bs = dk_bs; p.dk_ss = dk_ss; p.dv_bs = dv_bs; p.dv_ss = dv_ss;
+  p.dq = (bf16*)dq; p.dk = (bf16*)dk; p.dv = (bf16*)dv;
+  p.dq_bs = dq_bs; p.dq_ss = dq_ss; p.dk_bs = dk_bs; p.dk_ss = dk_ss; p.dv_bs = dv_bs; p.dv_ss = dv_ss;
   p.lse = lse; p.delta = delta; p.kmask = (const uint8_t*)kmask;
   p.B = B; p.nh = nh; p.nkv = nkv; p.Sq = Sq; p.Skv = Skv; p.hd = hd; p.causal = causal;
   p.scale_log2 = scale * LOG2E; p.scale = scale;
-  CB_CHECK_ARG((reinterpret_cast<uintptr_t>(dq_acc) & 7u) == 0, "attention bwd: dq_acc must be 8-byte aligned");
   // the dQ kernel streams 64-key K / V tiles against 128-query Q / dO tiles
   CUtensorMap tq128, tk64, tv64, tdo128;
   if ((rc = make_tmap_bf16_4d(&tq128, q, hd, nh, Sq, B, hd, q_ss, q_bs, 128))) return rc;

@@ -319,7 +319,7 @@ def attn_bwd(q, k, v, o, do, lse, *, causal: bool, kmask=None, scale: float | No
         scale = hd ** -0.5
     dev = q.device
     delta = torch.empty((B, nh, Sq), dtype=torch.float32, device=dev)
-    dq_acc = torch.empty((B, Sq, nh, hd), dtype=torch.float32, device=dev)   # every element written once
+    dq = dq if dq is not None else torch.empty((B, Sq, nh, hd), dtype=torch.bfloat16, device=dev)
     dk = dk if dk is not None else torch.empty((B, Skv, nkv, hd), dtype=torch.bfloat16, device=dev)
     dv = dv if dv is not None else torch.empty((B, Skv, nkv, hd), dtype=torch.bfloat16, device=dev)
     qb, qs = _bshd_strides(q, hd)
@@ -327,20 +327,16 @@ def attn_bwd(q, k, v, o, do, lse, *, causal: bool, kmask=None, scale: float | No
     vb, vs_ = _bshd_strides(v, hd)
     ob, os_ = _bshd_strides(o, hd)
     dob, dos = _bshd_strides(do, hd)
+    dqb, dqs = _bshd_strides(dq, hd)
     dkb, dks = _bshd_strides(dk, hd)
     dvb, dvs = _bshd_strides(dv, hd)
     if kmask is not None:
         kmask = kmask.contiguous()
         kmask = kmask.view(torch.uint8) if kmask.dtype == torch.bool else kmask.to(torch.uint8)
-    rc = _lib.load().cb_attn_bwd(ptr(q), ptr(k), ptr(v), ptr(o), ptr(do), ptr(lse), ptr(delta), ptr(dq_acc), ptr(dk),
+    rc = _lib.load().cb_attn_bwd(ptr(q), ptr(k), ptr(v), ptr(o), ptr(do), ptr(lse), ptr(delta), ptr(dq), ptr(dk),
                                  ptr(dv), ptr(kmask), B, nh, nkv, Sq, Skv, hd, qb, qs, kb, ks, vb, vs_, ob, os_, dob, dos,
-                                 dkb, dks, dvb, dvs, float(scale), int(causal), stream())
+                                 dqb, dqs, dkb, dks, dvb, dvs, float(scale), int(causal), stream())
     check(rc, "cb_attn_bwd")
-    if dq is None:
-        dq = torch.empty((B, Sq, nh, hd), dtype=torch.bfloat16, device=dev)
-    # dq may be a [B,Sq,nh,hd] view into a packed dQKV buffer: rows (b,s) at stride dq.stride(1)
-    assert dq.stride(3) == 1 and dq.stride(2) == hd and dq.stride(0) == Sq * dq.stride(1)
-    f32_to_bf16(dq_acc, dq, scale, cols=nh * hd, out_ld=dq.stride(1))
     return dq, dk, dv
 
 

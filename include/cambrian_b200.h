@@ -107,14 +107,13 @@ int64_t cb_norm_bwd_workspace_floats(int64_t rows, int C);
 int cb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, const void* kmask, int B, int nh,
                 int nkv, int Sq, int Skv, int hd, int64_t q_bs, int64_t q_ss, int64_t k_bs, int64_t k_ss,
                 int64_t v_bs, int64_t v_ss, int64_t o_bs, int64_t o_ss, float scale, int causal, void* stream);
-/* delta [B, nh, Sq] fp32 scratch; dq_acc [B, Sq, nh, hd] fp32 receives the unscaled sum dS K (multiply by `scale` when
- * converting, cb_f32_to_bf16); dk/dv written (bf16, strided).  Every output element has one writer (no atomics), so the
- * results are bit-identical from run to run. */
+/* delta [B, nh, Sq] fp32 scratch; dq/dk/dv written (bf16, strided, heads packed at hd: dq may be a view into a packed
+ * dQKV buffer).  Every output element has one writer (no atomics), so the results are bit-identical from run to run. */
 int cb_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
-                float* delta, float* dq_acc, void* dk, void* dv, const void* kmask, int B, int nh, int nkv, int Sq,
+                float* delta, void* dq, void* dk, void* dv, const void* kmask, int B, int nh, int nkv, int Sq,
                 int Skv, int hd, int64_t q_bs, int64_t q_ss, int64_t k_bs, int64_t k_ss, int64_t v_bs, int64_t v_ss,
-                int64_t o_bs, int64_t o_ss, int64_t do_bs, int64_t do_ss, int64_t dk_bs, int64_t dk_ss,
-                int64_t dv_bs, int64_t dv_ss, float scale, int causal, void* stream);
+                int64_t o_bs, int64_t o_ss, int64_t do_bs, int64_t do_ss, int64_t dq_bs, int64_t dq_ss,
+                int64_t dk_bs, int64_t dk_ss, int64_t dv_bs, int64_t dv_ss, float scale, int causal, void* stream);
 
 /* ---- elementwise / gather / reduction kernels (HBM-bound) -------------------------------------- */
 /* y = act(x), dx = dy * act'(x); n elements (n % 8 == 0).  nn.GELU of vision_sampler.py:241, cambrian_arch.py:49,56 */
