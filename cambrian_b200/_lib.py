@@ -75,6 +75,9 @@ SIGNATURES = {
     "cb_tower_combine_fwd": (_i, [_vp, _i, _vpp, _vp, _vp, _i64, _i, _i, _vp]),
     "cb_tower_combine_bwd": (_i, [_vp, _i, _vpp, _vp, _vpp, _vp, _i64, _i, _i, _vp]),
     "cb_bilinear_bwd": (_i, [_vp, _vp] + [_i] * 6 + [_vp]),
+    "cb_nf4_quantize": (_i, [_vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "cb_gemv_nf4": (_i, [_vp, _vp, _i, _i, _i, _i64, _i64, _i, _ip, _vpp, _vpp, _vpp, _vpp, _vp, _vp, _i64, _i, _vp]),
+    "cb_nf4_dequant": (_i, [_vp, _i, _i, _i, _ip, _vpp, _vpp, _vpp, _vpp, _vp]),
 }
 
 _lib = None

@@ -8,8 +8,9 @@ the unchanged `PreTrainedModel.from_pretrained`.  This file adds the three refer
     (`safe_save_model_for_hf_trainer`, train_fsdp.py:249-283; key filter :255);
   * `load_mm_projector` — the `mm_projector.bin` overlay on top of a base LLM (model/builder.py:107-114) and the
     `pretrain_mm_mlp_adapter` path of `initialize_vision_modules` (cambrian_arch.py:183-200, strict per sub-module);
-  * `load_pretrained_model` — the loader the eval / serve harness calls (model/builder.py:29-175), bf16 on one GPU.
-    LoRA merging and 4/8-bit quantised loading are outside the hot path and raise NotImplementedError.
+  * `load_pretrained_model` — the loader the eval / serve harness calls (model/builder.py:29-175), bf16 on one GPU, or
+    with `load_4bit=True` the decoder projections in NF4 (quant.py).  LoRA merging and 8-bit (LLM.int8) loading raise
+    NotImplementedError.
 """
 from __future__ import annotations
 
@@ -70,12 +71,14 @@ def load_mm_projector(model, path_or_state, strict_submodules: bool = False):
 def load_pretrained_model(model_path, model_base=None, model_name="cambrian", load_8bit=False, load_4bit=False,
                           device="cuda", dtype=torch.bfloat16, load_tokenizer=True, **kwargs):
     """model/builder.py:29-175 for the LLaMA-family Cambrian checkpoints: returns (tokenizer, model, image_processor list,
-    context_len).  `model_base` + `<model_path>/mm_projector.bin` is the connector-only layout (:103-114)."""
+    context_len).  `model_base` + `<model_path>/mm_projector.bin` is the connector-only layout (:103-114).
+    load_4bit=True (:37-44): the checkpoint loads in bf16 on the CPU, the seven projections of every decoder layer are
+    quantised to NF4 layer by layer on `device` (quant.quantize_decoder_nf4_), everything else moves there in bf16."""
     from transformers import AutoConfig, AutoTokenizer
 
     from .model.language_model.cambrian_llama import CambrianLlamaForCausalLM
-    if load_8bit or load_4bit:
-        raise NotImplementedError("bitsandbytes-quantised loading is not part of this path (bf16 only)")
+    if load_8bit:
+        raise NotImplementedError("8-bit (LLM.int8) loading is not supported; load_4bit=True gives NF4 decoder weights")
     if "lora" in model_name.lower():
         raise NotImplementedError("LoRA merging (builder.py:56-92) is outside the hot path: merge with the reference tools first")
     if "mistral" in model_name.lower() or "phi3" in model_name.lower():
@@ -88,6 +91,9 @@ def load_pretrained_model(model_path, model_base=None, model_name="cambrian", lo
         load_mm_projector(model, os.path.join(model_path, "mm_projector.bin"))
     else:
         model = CambrianLlamaForCausalLM.from_pretrained(model_path, torch_dtype=dtype, **kwargs)
+    if load_4bit:
+        from .quant import quantize_decoder_nf4_
+        quantize_decoder_nf4_(model, device)
     model.to(device=device, dtype=dtype)
     towers = model.get_vision_tower_aux_list() or []
     for t in towers:

@@ -105,6 +105,12 @@ int tower_combine_fwd_launch(const void*, int, const void* const*, const void*, 
 int tower_combine_bwd_launch(const void*, int, const void* const*, const void*, void* const*, void*, long long, int, int,
                              cudaStream_t);
 int bilinear_bwd_launch(const void*, void*, int, int, int, int, int, int, cudaStream_t);
+int nf4_quantize_launch(const void*, int, int, float*, long long, void*, void*, float*, float*, cudaStream_t);
+int gemv_nf4_launch(const void*, void*, int, int, int, long long, long long, int, const int*, const void* const*,
+                    const void* const*, const void* const*, const void* const*, const void*, const void*, long long, int,
+                    cudaStream_t);
+int nf4_dequant_launch(void*, int, int, int, const int*, const void* const*, const void* const*, const void* const*,
+                       const void* const*, cudaStream_t);
 
 }  // namespace cb
 
@@ -335,6 +341,20 @@ int cb_tower_combine_bwd(const void* logits, int ld_logits, const void* const* a
 }
 int cb_bilinear_bwd(const void* dout, void* din, int B, int h, int w, int th, int tw, int C, void* stream) {
   return cb::bilinear_bwd_launch(dout, din, B, h, w, th, tw, C, ST(stream));
+}
+int cb_nf4_quantize(const void* w, int N, int K, float* absmax_ws, int64_t ws_floats, void* packed, void* qabsmax,
+                    float* absmax2, float* offset, void* stream) {
+  return cb::nf4_quantize_launch(w, N, K, absmax_ws, ws_floats, packed, qabsmax, absmax2, offset, ST(stream));
+}
+int cb_gemv_nf4(const void* x, void* y, int M, int N, int K, int64_t ldx, int64_t ldy, int nseg, const int32_t* seg_row0,
+                const void* const* packed, const void* const* qabsmax, const void* const* absmax2, const void* const* offset,
+                const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream) {
+  return cb::gemv_nf4_launch(x, y, M, N, K, ldx, ldy, nseg, seg_row0, packed, qabsmax, absmax2, offset, bias, residual, ldr,
+                             out_fp32, ST(stream));
+}
+int cb_nf4_dequant(void* out, int N, int K, int nseg, const int32_t* seg_row0, const void* const* packed,
+                   const void* const* qabsmax, const void* const* absmax2, const void* const* offset, void* stream) {
+  return cb::nf4_dequant_launch(out, N, K, nseg, seg_row0, packed, qabsmax, absmax2, offset, ST(stream));
 }
 
 }  // extern "C"

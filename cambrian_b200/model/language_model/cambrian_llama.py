@@ -158,6 +158,7 @@ class CBLlamaDecoderLayer(nn.Module):
         self.mlp = CBLlamaMLP(config)
         self.input_layernorm = CBRMSNorm(config.hidden_size, config.rms_norm_eps)
         self.post_attention_layernorm = CBRMSNorm(config.hidden_size, config.rms_norm_eps)
+        self._nf4 = None        # NF4 projections (quant.quantize_decoder_nf4_): the bf16 weights are freed then
 
     def _fused(self):
         a, m = self.self_attn, self.mlp
@@ -166,6 +167,11 @@ class CBLlamaDecoderLayer(nn.Module):
         return fuse_rows(qkv), fuse_rows(gu), _FusedGrad(qkv), _FusedGrad(gu)
 
     def forward(self, x, rt):
+        if self._nf4 is not None:
+            if torch.is_grad_enabled():
+                raise NotImplementedError("a 4-bit (NF4) model is inference-only: training quantised weights (QLoRA) is "
+                                          "not supported; run it under torch.no_grad()")
+            return self.infer(x, rt, None)
         a, m = self.self_attn, self.mlp
         qkv_w, gu_w, g_qkv, g_gu = self._fused()
         meta = dict(nh=self.nh, nkv=self.nkv, hd=self.hd, eps=self.input_layernorm.variance_epsilon,
@@ -179,32 +185,48 @@ class CBLlamaDecoderLayer(nn.Module):
 
     @torch.no_grad()
     def infer(self, x, rt, cache):
-        """KV-cache path (prefill and decode): same kernels, K/V appended to the per-layer cache."""
+        """KV-cache path (prefill and decode): same kernels, K/V appended to the per-layer cache.  cache=None: causal
+        attention over the sequence itself (no-grad forward of a 4-bit model).  NF4 layers run their projections through
+        ops.nf4_linear / ops.nf4_mlp_gate_up."""
         a, m = self.self_attn, self.mlp
-        qkv_w, gu_w, _, _ = self._fused()
+        nf4 = self._nf4
+        if nf4 is None:
+            qkv_w, gu_w, _, _ = self._fused()
         B, S, H = x.shape
         nh, nkv, hd = self.nh, self.nkv, self.hd
         rows = B * S
         x2 = x.reshape(rows, H)
         h = ops.rmsnorm_fwd(x2, self.input_layernorm.weight, self.input_layernorm.variance_epsilon, rt["hf_cast"])
-        qkv = ops.gemm(h, qkv_w)
+        qkv = ops.nf4_linear(h, nf4["qkv"]) if nf4 is not None else ops.gemm(h, qkv_w)
         ops.rope_(qkv, rt["pos"], rt["cos"], rt["sin"], nh + nkv, hd)
-        kc, vc = cache.k[self.layer_idx], cache.v[self.layer_idx]
         q = qkv[:, : nh * hd].view(B, S, nh, hd)
-        if cache.slot is not None:
+        k_new = qkv[:, nh * hd:(nh + nkv) * hd].view(B, S, nkv, hd)
+        v_new = qkv[:, (nh + nkv) * hd:].view(B, S, nkv, hd)
+        if cache is None:
+            attn = ops.attn_fwd(q, k_new, v_new, causal=True, kmask=rt["kmask"])
+        elif cache.slot is not None:
             # static-shape decode step (CUDA-graph replay): the write slot is a DEVICE index, attention runs over the whole
             # cache buffer and the validity mask (updated on the device) hides the slots not written yet
-            kc.index_copy_(1, cache.slot, qkv[:, nh * hd:(nh + nkv) * hd].view(B, S, nkv, hd))
-            vc.index_copy_(1, cache.slot, qkv[:, (nh + nkv) * hd:].view(B, S, nkv, hd))
+            kc, vc = cache.k[self.layer_idx], cache.v[self.layer_idx]
+            kc.index_copy_(1, cache.slot, k_new)
+            vc.index_copy_(1, cache.slot, v_new)
             attn = ops.attn_fwd(q, kc, vc, causal=False, kmask=rt["kmask"])
         else:
+            kc, vc = cache.k[self.layer_idx], cache.v[self.layer_idx]
             t0 = cache.length
-            kc[:, t0:t0 + S].copy_(qkv[:, nh * hd:(nh + nkv) * hd].view(B, S, nkv, hd))   # cache append (memory plumbing)
-            vc[:, t0:t0 + S].copy_(qkv[:, (nh + nkv) * hd:].view(B, S, nkv, hd))
+            kc[:, t0:t0 + S].copy_(k_new)   # cache append (memory plumbing)
+            vc[:, t0:t0 + S].copy_(v_new)
             attn = ops.attn_fwd(q, kc[:, : t0 + S], vc[:, : t0 + S], causal=True, kmask=rt["kmask"])
-        x1 = ops.gemm(attn.view(rows, nh * hd), a.o_proj.weight, residual=x2)
+        attn2 = attn.view(rows, nh * hd)
+        if nf4 is not None:
+            x1 = ops.nf4_linear(attn2, nf4["o"], residual=x2)
+        else:
+            x1 = ops.gemm(attn2, a.o_proj.weight, residual=x2)
         h2 = ops.rmsnorm_fwd(x1, self.post_attention_layernorm.weight, self.post_attention_layernorm.variance_epsilon,
                              rt["hf_cast"])
+        if nf4 is not None:
+            _, act = ops.nf4_mlp_gate_up(h2, nf4["gate_up"])
+            return ops.nf4_linear(act, nf4["down"], residual=x1).view(B, S, H)
         _, act = ops.mlp_gate_up(h2, gu_w)
         return ops.gemm(act, m.down_proj.weight, residual=x1).view(B, S, H)
 
@@ -406,6 +428,13 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
 
     def get_model(self):
         return self.model
+
+    def save_pretrained(self, *args, **kwargs):
+        from ...quant import is_quantized
+        if is_quantized(self):
+            raise NotImplementedError("save_pretrained of a 4-bit (NF4) model is not supported: its decoder projections "
+                                      "hold no bf16 weights; save the bf16 checkpoint it was loaded from instead")
+        return super().save_pretrained(*args, **kwargs)
 
     def get_input_embeddings(self):
         return self.model.embed_tokens

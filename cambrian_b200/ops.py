@@ -707,3 +707,61 @@ def mlp_gate_up(h2d, w_gu):
         return gemm_swiglu(h2d, w_gu)
     gu = gemm(h2d, w_gu)
     return gu, swiglu_fwd(gu[:, :I], gu[:, I:])
+
+
+# ------------------------------------------------------------------------------------------------
+# NF4 decoder weights (load_4bit; the format lives in quant.py)
+# ------------------------------------------------------------------------------------------------
+def nf4_quantize(w, workspace, packed, qabsmax, absmax2, offset):
+    """Quantise one contiguous bf16 [N, K] weight into caller-allocated NF4 buffers (workspace: fp32, >= N*K/64)."""
+    _chk(w, "w")
+    N, K = w.shape
+    check(_lib.load().cb_nf4_quantize(ptr(w), N, K, ptr(workspace), workspace.numel(), ptr(packed), ptr(qabsmax),
+                                      ptr(absmax2), ptr(offset), stream()), "cb_nf4_quantize")
+
+
+def _nf4_segments(qw):
+    row0, packed, qabsmax, absmax2, offset = qw.segment_arrays()
+    return len(row0), int_array(row0), ptr_array(packed), ptr_array(qabsmax), ptr_array(absmax2), ptr_array(offset)
+
+
+def gemv_nf4(x, qw, bias=None, residual=None, out=None, out_dtype=torch.bfloat16) -> torch.Tensor:
+    """y[M, N] = x[M, K] @ W~^T (+ bias) (+ residual) for M <= 8 on an NF4 projection (quant.NF4Projection)."""
+    _require_cuda_bf16(x, bias, residual)
+    M = x.shape[0]
+    if out is None:
+        out = torch.empty((M, qw.N), dtype=out_dtype, device=x.device)
+    if out.dtype not in (torch.bfloat16, torch.float32) or out.stride(-1) != 1 or out.shape != (M, qw.N):
+        raise ValueError("gemv_nf4: out must be a bf16 / fp32 [M, N] tensor with contiguous rows")
+    if residual is not None and (residual.shape != out.shape or residual.stride(-1) != 1):
+        raise ValueError("gemv_nf4: residual must match the output shape")
+    if x.shape[1] != qw.K or x.stride(1) != 1:
+        raise ValueError(f"gemv_nf4: x {tuple(x.shape)} does not match K = {qw.K}")
+    check(_lib.load().cb_gemv_nf4(ptr(x), ptr(out), M, qw.N, qw.K, x.stride(0), out.stride(0), *_nf4_segments(qw),
+                                  ptr(bias), ptr(residual), residual.stride(0) if residual is not None else 0,
+                                  int(out.dtype == torch.float32), stream()), "cb_gemv_nf4")
+    return out
+
+
+def nf4_dequant(qw) -> torch.Tensor:
+    """W~ [N, K] bf16 of an NF4 projection, written into (a view of) its model-owned scratch buffer."""
+    out = qw.scratch[: qw.N * qw.K].view(qw.N, qw.K)
+    check(_lib.load().cb_nf4_dequant(ptr(out), qw.N, qw.K, *_nf4_segments(qw), stream()), "cb_nf4_dequant")
+    return out
+
+
+def nf4_linear(x, qw, residual=None, out=None, out_dtype=torch.bfloat16) -> torch.Tensor:
+    """y = x @ W~^T (+ residual) on an NF4 projection: the NF4 GEMV for M <= 8 rows (decode), otherwise W~ is
+    dequantised into the model's scratch buffer and the bf16 GEMM runs on it (prefill, batches above 8)."""
+    if x.shape[0] <= 8:
+        return gemv_nf4(x, qw, residual=residual, out=out, out_dtype=out_dtype)
+    return gemm(x, nf4_dequant(qw), residual=residual, out=out, out_dtype=out_dtype)
+
+
+def nf4_mlp_gate_up(h2d, qw):
+    """`mlp_gate_up` on the fused NF4 gate|up projection: (gu [M, 2F], act = silu(gate) * up)."""
+    if h2d.shape[0] <= 8:
+        gu = gemv_nf4(h2d, qw)
+        I = qw.N // 2
+        return gu, swiglu_fwd(gu[:, :I], gu[:, I:])
+    return mlp_gate_up(h2d, nf4_dequant(qw))

@@ -249,6 +249,27 @@ int cb_tower_combine_bwd(const void* logits, int ld_logits, const void* const* a
 /* adjoint of cb_bilinear on contiguous grids: dout [B, th, tw, C] -> din [B, h, w, C] (backward of the query-grid resize
  * cambrian_arch.py:394-401 and of the towers' token interpolation, clip_encoder.py:83-88 and siblings); deterministic */
 int cb_bilinear_bwd(const void* dout, void* din, int B, int h, int w, int th, int tw, int C, void* stream);
+/* 4-bit NF4 decoder weights with double-quantised scales, the `load_4bit` path of model/builder.py:37-44 (bitsandbytes
+ * NF4 + double quantisation there; the format is defined in cambrian_b200/quant.py).  Blocks of 64 row-major elements of
+ * one Linear weight W [N, K] (K % 64 == 0); packed [N, K/2] uint8 codes (element 2j in the high nibble), qabsmax [N*K/64]
+ * uint8 indices into the signed dynamic map, absmax2 [ceil(N*K/64 / 256)] fp32 group scales, offset [1] fp32.
+ * Dequantised weight: w~ = bf16(c[code] * (map[qabsmax] * absmax2 + offset)), no FMA contraction.
+ *
+ * cb_nf4_quantize: quantise one bf16 W [N, K] on the device; absmax_ws is caller-provided fp32 scratch of >= N*K/64
+ * floats.  Deterministic (fixed-order reductions), no host synchronisation. */
+int cb_nf4_quantize(const void* w, int N, int K, float* absmax_ws, int64_t ws_floats, void* packed, void* qabsmax,
+                    float* absmax2, float* offset, void* stream);
+/* Decode-shaped projection on NF4 weights, M <= 8 rows: y[M,N] = x[M,K] W~[N,K]^T (+ bias[N]) (+ residual[M,N]), y bf16 or
+ * fp32, fp32 accumulation — the NF4 counterpart of cb_gemv_bf16 for the KV-cache decode step.  W~ may be a fused
+ * projection (q|k|v, gate|up) of up to 3 separately quantised row segments: HOST arrays of nseg entries, segment i covers
+ * rows [seg_row0[i], seg_row0[i+1]) (seg_row0[0] = 0) and carries its own packed / qabsmax / absmax2 / offset. */
+int cb_gemv_nf4(const void* x, void* y, int M, int N, int K, int64_t ldx, int64_t ldy, int nseg, const int32_t* seg_row0,
+                const void* const* packed, const void* const* qabsmax, const void* const* absmax2, const void* const* offset,
+                const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream);
+/* W~ of a segmented NF4 weight (same segment table as cb_gemv_nf4) written as bf16 [N, K] into caller-provided scratch,
+ * bitwise equal to the definition above: the larger-batch path runs the bf16 GEMM on it. */
+int cb_nf4_dequant(void* out, int N, int K, int nseg, const int32_t* seg_row0, const void* const* packed,
+                   const void* const* qabsmax, const void* const* absmax2, const void* const* offset, void* stream);
 
 #ifdef __cplusplus
 }
