@@ -56,6 +56,7 @@ SIGNATURES = {
     "cb_cross_entropy_ex": (_i, [_vp] * 4 + [_i64, _i64, _i64, _f, _vp, _i, _i64, _vp]),
     "cb_adamw": (_i, [_vp] * 5 + [_i64] + [_f] * 5 + [_i, _f, _vp]),
     "cb_adamw_ex": (_i, [_vp] * 5 + [_i64] + [_f] * 5 + [_i, _f, _vp, _i, _vp]),
+    "cb_adamw_host": (_i, [_vp] * 5 + [_i64] + [_f] * 5 + [_i, _f, _vp, _i, _vp]),
     "cb_gemv_bf16": (_i, [_vp, _vp, _vp, _i, _i, _i, _i64, _i64, _i64, _vp, _vp, _i64, _i, _vp]),
     "cb_allreduce_symm_bf16": (_i, [C.c_uint64, _vp, _vp, _i64, _i64, _i, _i, C.c_uint32, _i, _vp]),
     "cb_embed_grad_sorted": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _i64, _vp]),

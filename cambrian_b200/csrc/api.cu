@@ -84,6 +84,8 @@ int cross_entropy_launch(void*, const long long*, float*, float*, long long, lon
                          int, long long, cudaStream_t);
 int adamw_launch(float*, float*, float*, const void*, void*, long long, float, float, float, float, float, int, float,
                  const float*, int, cudaStream_t);
+int adamw_host_launch(float*, float*, float*, const void*, void*, long long, float, float, float, float, float, int, float,
+                      const float*, int, cudaStream_t);
 int sumsq_launch(const void*, long long, float*, float*, long long, int, cudaStream_t);
 int gemv_bf16_launch(const void*, const void*, void*, int, int, int, long long, long long, long long, const void*, const void*,
                      long long, int, cudaStream_t);
@@ -308,6 +310,11 @@ int cb_adamw_ex(float* p, float* m, float* v, const void* g, void* p16, int64_t 
                 void* stream) {
   return cb::adamw_launch(p, m, v, g, p16, n, lr, beta1, beta2, eps, weight_decay, step, grad_scale, clip_coef, background,
                           ST(stream));
+}
+int cb_adamw_host(float* p, float* m, float* v, const void* g, void* p16, int64_t n, float lr, float beta1, float beta2,
+                  float eps, float weight_decay, int step, float grad_scale, const float* clip_coef, int ctas, void* stream) {
+  return cb::adamw_host_launch(p, m, v, g, p16, n, lr, beta1, beta2, eps, weight_decay, step, grad_scale, clip_coef, ctas,
+                               ST(stream));
 }
 int cb_embed_grad_sorted(const void* dout, const int64_t* keys, const int32_t* order, void* d_embed, int64_t n, int H,
                          int64_t vocab, void* stream) {

@@ -22,7 +22,10 @@ buffers for bf16 gradients, fp32 master weights and fp32 Adam moments:
     AdamW.  Because no update may start before the global norm is known, with clipping the updates run after backward, in
     the order the NEXT forward consumes the parameters, and each consumer waits only for its own bucket's event
     (`autograd._await`): the optimizer hides under the frozen towers and the first decoder layers of the next step.
-    Without clipping each bucket is updated as soon as it is reduced, under the rest of backward.
+    Without clipping each bucket is updated as soon as it is reduced, under the rest of backward;
+  * `offload_optimizer=True` (DeepSpeed's `offload_optimizer`, scripts/zero3_offload.json) keeps the fp32 master and
+    moments in registered host memory: the device holds 4 B per trainable parameter instead of 16, and the update kernel
+    (`ops.adamw_host`) streams the state over PCIe, same arithmetic on the GPU, same schedule and streams as above.
 
 Gradient contributions are counted per parameter: the counts are structural (one per weight-gradient GEMM site, lm_head
 notifies once per step however many row chunks it processes), learned on the first step and verified equal across ranks
@@ -34,6 +37,7 @@ and steps HF Trainer's AdamW (cambrian_trainer.py:242-381).
 from __future__ import annotations
 
 import functools
+import weakref
 
 import torch
 import torch.distributed as dist
@@ -73,7 +77,7 @@ class TrainEngine:
                  weight_decay: float = 0.0, bucket_mb: float = 256.0, process_group=None, overlap: bool = True,
                  zero_stage: int = 0, max_grad_norm: float | None = None, mm_projector_lr: float | None = None,
                  mm_vision_sampler_lr: float | None = None, lr_lambda=None, loss_scale: float = 1.0,
-                 background_optimizer: bool = False, collective: str = "nccl"):
+                 background_optimizer: bool = False, collective: str = "nccl", offload_optimizer: bool = False):
         if zero_stage not in (0, 2):
             raise ValueError("zero_stage must be 0 or 2")
         from .quant import is_quantized
@@ -166,7 +170,11 @@ class TrainEngine:
             p._cb_engine = self
             p._cb_bucket = self._bucket_of[i]
             p.grad = None
-        # ---- optimizer state: whole buffer (DDP) or this rank's piece of every bucket (ZeRO-2)
+        # ---- optimizer state: whole buffer (DDP) or this rank's piece of every bucket (ZeRO-2); on the device, or in
+        #      registered host memory with offload_optimizer
+        self.offload = bool(offload_optimizer)
+        self._closed = False
+        self._host_finalizer = None
         self.piece_base = None
         if zero_stage == 2:
             self.piece_base, n_state = [], 0
@@ -174,17 +182,22 @@ class TrainEngine:
                 self.piece_base.append(n_state)
                 n_state += (e - s) // self.world
             self.shard = n_state
-            self.master = torch.empty(n_state, dtype=torch.float32, device=dev)
-            for b, (s, e, _) in enumerate(self.buckets):
-                lo, hi = self._piece(b)
-                self.master[self.piece_base[b]:self.piece_base[b] + hi - lo].copy_(self.flat_p[lo:hi])
+            if not self.offload:
+                self.master = torch.empty(n_state, dtype=torch.float32, device=dev)
+                for b, (s, e, _) in enumerate(self.buckets):
+                    lo, hi = self._piece(b)
+                    self.master[self.piece_base[b]:self.piece_base[b] + hi - lo].copy_(self.flat_p[lo:hi])
             self.shard_g = torch.zeros(n_state, dtype=torch.bfloat16, device=dev)
         else:
             self.shard = 0
             n_state = total
-            self.master = self.flat_p.float()
-        self.exp_avg = torch.zeros(n_state, dtype=torch.float32, device=dev)
-        self.exp_avg_sq = torch.zeros(n_state, dtype=torch.float32, device=dev)
+            if not self.offload:
+                self.master = self.flat_p.float()
+        if self.offload:
+            self._init_host_state(n_state)
+        else:
+            self.exp_avg = torch.zeros(n_state, dtype=torch.float32, device=dev)
+            self.exp_avg_sq = torch.zeros(n_state, dtype=torch.float32, device=dev)
         self._static_segments = [self._segments(b, ()) for b in range(len(self.buckets))]
         # ---- clipping state (device side; no host sync)
         self._sumsq = torch.zeros(1, dtype=torch.float32, device=dev)   # reset by the clip kernel itself (stream-ordered)
@@ -213,6 +226,31 @@ class TrainEngine:
         if hasattr(model, "prepare_inputs_labels_for_multimodal"):
             model._cb_param_sync = self.wait_for_params     # kept for API compatibility: a full wait
             model._cb_loss_scale = self.loss_scale
+
+    def _init_host_state(self, n_state):
+        """fp32 master and moments as CPU tensors, registered with CUDA when the model is on the GPU (offload_optimizer).
+        The master is filled one bucket (ZeRO-2: one piece) at a time through a device scratch of that size: a full-size
+        fp32 copy on the device is exactly what offloading exists to avoid."""
+        self.master = torch.empty(n_state, dtype=torch.float32)
+        self.exp_avg = torch.zeros(n_state, dtype=torch.float32)
+        self.exp_avg_sq = torch.zeros(n_state, dtype=torch.float32)
+        if self.flat_p.is_cuda:
+            registered = []
+            try:
+                for t in (self.master, self.exp_avg, self.exp_avg_sq):
+                    registered.append(ops.host_register(t))
+            except Exception:
+                _release_host_state(self.flat_p.device, registered)
+                raise
+            # unregisters before the tensors can be freed: on close() or when the engine is collected
+            self._host_finalizer = weakref.finalize(self, _release_host_state, self.flat_p.device, registered)
+        pieces = [self._piece(b) if self.zero_stage == 2 else self.buckets[b][:2] for b in range(len(self.buckets))]
+        scratch = torch.empty(max(hi - lo for lo, hi in pieces), dtype=torch.float32, device=self.flat_p.device)
+        for b, (lo, hi) in enumerate(pieces):
+            at = self.piece_base[b] if self.zero_stage == 2 else lo
+            sc = scratch[:hi - lo]
+            sc.copy_(self.flat_p[lo:hi])
+            self.master[at:at + hi - lo].copy_(sc)
 
     # ---- layout helpers --------------------------------------------------------------------------------------------
     def _piece(self, b):
@@ -253,8 +291,8 @@ class TrainEngine:
             self._remaining = [sum(1 for i in idx if self._expected[i] > 0) for (_, _, idx) in self.buckets]
 
     def _opt(self):
-        if self._opt_stream is None and self.master.is_cuda:
-            self._opt_stream = torch.cuda.Stream(device=self.master.device)
+        if self._opt_stream is None and self.flat_p.is_cuda:
+            self._opt_stream = torch.cuda.Stream(device=self.flat_p.device)
         return self._opt_stream
 
     def _launch_bucket(self, b):
@@ -363,6 +401,10 @@ class TrainEngine:
                 run()
 
     def _adamw(self, master, m, v, g, p16, lr, wd, step, coef):
+        if self.offload:
+            ops.adamw_host(master, m, v, g, p16, lr, self.betas[0], self.betas[1], self.eps, wd, step,
+                           grad_scale=1.0 / self.world, clip_coef=coef)
+            return
         ops.adamw(master, m, v, g, p16, lr, self.betas[0], self.betas[1], self.eps, wd, step,
                   grad_scale=1.0 / self.world, clip_coef=coef, background=self.background)
 
@@ -431,7 +473,7 @@ class TrainEngine:
         self._expected = list(self._writes)
         ok = True
         if self.world > 1:
-            dev = self.master.device
+            dev = self.flat_p.device
             t = torch.tensor(self._expected, dtype=torch.int64, device=dev)
             lo, hi = t.clone(), t.clone()
             dist.all_reduce(lo, op=dist.ReduceOp.MIN, group=self.pg)
@@ -443,6 +485,8 @@ class TrainEngine:
             warnings.warn("TrainEngine: gradient-contribution counts differ between ranks; collectives stay serial")
 
     def step(self):
+        if self._closed:
+            raise RuntimeError("TrainEngine: step() after close(): the host-resident optimizer state was released")
         first = self._expected is None
         self._finalize_unwritten()
         if first:
@@ -454,7 +498,7 @@ class TrainEngine:
             raise RuntimeError(f"TrainEngine: {self.names[i]} received {self._writes[i]} gradient contributions this step, "
                                f"{self._expected[i]} were learned on step 1; call engine.relearn() before a step whose "
                                "graph differs (it then runs without overlap)")
-        side = self.master.is_cuda
+        side = self.flat_p.is_cuda
         order = list(reversed(range(len(self.buckets))))
         for b in order:                                   # collectives not launched during backward: fixed order
             if not self._launched[b]:
@@ -522,5 +566,23 @@ class TrainEngine:
         return out.loss
 
     def state_bytes(self):
+        """Device bytes of training state: bf16 weights and gradients, plus the fp32 master and moments unless offloaded."""
         opt = (self.shard if self.zero_stage == 2 else self.total) * 12
-        return self.total * 4 + opt
+        return self.total * 4 + (0 if self.offload else opt)
+
+    def host_state_bytes(self):
+        """Host bytes of the offloaded fp32 master and moments (0 without offload_optimizer)."""
+        return 3 * 4 * self.master.numel() if self.offload else 0
+
+    def close(self):
+        """Unregister the host-resident optimizer state (after the device has finished with it).  Idempotent, and run
+        when the engine is garbage-collected; step() raises afterwards.  The host tensors stay readable."""
+        self._closed = True
+        if self._host_finalizer is not None:
+            self._host_finalizer()
+
+
+def _release_host_state(device, tensors):
+    torch.cuda.synchronize(device)          # no update may still be reading or writing them
+    for t in tensors:
+        ops.host_unregister(t)

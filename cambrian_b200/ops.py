@@ -569,6 +569,33 @@ def adamw(p32, m, v, g16, p16, lr, beta1, beta2, eps, wd, step: int, grad_scale:
                                   int(background), stream()), "cb_adamw_ex")
 
 
+def adamw_host(p32, m, v, g16, p16, lr, beta1, beta2, eps, wd, step: int, grad_scale: float = 1.0, clip_coef=None,
+               ctas: int = 0):
+    """`adamw` with p32, m, v in host memory registered by `host_register` (the update streams them over PCIe and is
+    bitwise equal to `adamw`); g16, p16 and clip_coef on the device.  ctas: grid size, 0 = the measured default."""
+    check(_lib.load().cb_adamw_host(ptr(p32), ptr(m), ptr(v), ptr(g16), ptr(p16), p32.numel(), float(lr), float(beta1),
+                                    float(beta2), float(eps), float(wd), int(step), float(grad_scale), ptr(clip_coef),
+                                    int(ctas), stream()), "cb_adamw_host")
+
+
+_HOST_REGISTER_PORTABLE, _HOST_REGISTER_MAPPED = 1, 2
+
+
+def host_register(t):
+    """Page-lock a contiguous CPU tensor's own bytes and map them into the device address space (cudaHostRegister, mapped
+    | portable), for `adamw_host`.  torch's pinned allocator would round a 33 GB request up to 64 GB; this pins exactly
+    the tensor.  Call `host_unregister` before the tensor is freed."""
+    if t.is_cuda or not t.is_contiguous():
+        raise ValueError("host_register: expects a contiguous CPU tensor")
+    torch.cuda.check_error(torch.cuda.cudart().cudaHostRegister(
+        t.data_ptr(), t.numel() * t.element_size(), _HOST_REGISTER_PORTABLE | _HOST_REGISTER_MAPPED))
+    return t
+
+
+def host_unregister(t):
+    torch.cuda.check_error(torch.cuda.cudart().cudaHostUnregister(t.data_ptr()))
+
+
 def sumsq_accumulate(g16, acc, ws, background: bool = True):
     """acc[0] += sum(g16^2) (deterministic); g16 bf16 contiguous with numel % 8 == 0; ws fp32 scratch (>= 4096)."""
     _require_cuda_bf16(g16)

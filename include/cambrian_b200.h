@@ -211,6 +211,14 @@ int cb_adamw(float* p, float* m, float* v, const void* g, void* p16, int64_t n, 
 int cb_adamw_ex(float* p, float* m, float* v, const void* g, void* p16, int64_t n, float lr, float beta1, float beta2,
                 float eps, float weight_decay, int step, float grad_scale, const float* clip_coef, int background,
                 void* stream);
+/* cb_adamw_ex with the fp32 state in HOST memory (DeepSpeed's `offload_optimizer`, scripts/zero3_offload.json), the
+ * arithmetic still on the GPU and bitwise equal to cb_adamw_ex: p, m, v are host memory registered with CUDA and mapped
+ * (cudaHostRegister with cudaHostRegisterMapped), read and written over PCIe in one pass; g, p16 (and clip_coef) are
+ * device memory.  The one exception to "every pointer is a device pointer".  Every pointer's placement is checked before
+ * the launch: a pointer in the wrong kind of memory returns CB_ERR_INVALID naming the argument.  ctas: blocks of the
+ * PCIe-bound grid (0 = default); 128-thread blocks without shared memory that fit next to a resident GEMM CTA. */
+int cb_adamw_host(float* p, float* m, float* v, const void* g, void* p16, int64_t n, float lr, float beta1, float beta2,
+                  float eps, float weight_decay, int step, float grad_scale, const float* clip_coef, int ctas, void* stream);
 /* Deterministic gradient of the embedding rows (backward of embed_tokens inside cb_embed_splice): rows of dout [n, H] with
  * equal keys[t] (token id; >= vocab = no gradient, e.g. the image span) are summed in position order by one block and
  * written once to d_embed [vocab, H] (pre-zeroed).  `order` = positions stably sorted by key.  Replaces the racing
