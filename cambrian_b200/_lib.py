@@ -79,6 +79,10 @@ SIGNATURES = {
     "cb_nf4_quantize": (_i, [_vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "cb_gemv_nf4": (_i, [_vp, _vp, _i, _i, _i, _i64, _i64, _i, _ip, _vpp, _vpp, _vpp, _vpp, _vp, _vp, _i64, _i, _vp]),
     "cb_nf4_dequant": (_i, [_vp, _i, _i, _i, _ip, _vpp, _vpp, _vpp, _vpp, _vp]),
+    "cb_int8_quantize_weight": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp]),
+    "cb_int8_quantize_act": (_i, [_vp, _i, _i, _i64, _f, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "cb_gemv_int8": (_i, [_vp] * 5 + [_i64, _vp, _vp, _vp, _i, _i, _i, _i64, _vp, _vp, _i64, _i, _vp]),
+    "cb_gemm_int8": (_i, [_vp] * 5 + [_i64, _vp, _vp, _vp, _i, _i, _i, _i64, _vp, _vp, _i64, _i, _vp]),
 }
 
 _lib = None

@@ -9,8 +9,8 @@ the unchanged `PreTrainedModel.from_pretrained`.  This file adds the three refer
   * `load_mm_projector` — the `mm_projector.bin` overlay on top of a base LLM (model/builder.py:107-114) and the
     `pretrain_mm_mlp_adapter` path of `initialize_vision_modules` (cambrian_arch.py:183-200, strict per sub-module);
   * `load_pretrained_model` — the loader the eval / serve harness calls (model/builder.py:29-175), bf16 on one GPU, or
-    with `load_4bit=True` the decoder projections in NF4 (quant.py).  LoRA merging and 8-bit (LLM.int8) loading raise
-    NotImplementedError.
+    with `load_4bit=True` the decoder projections in NF4 (quant.py), with `load_8bit=True` in LLM.int8
+    (quant_int8.py).  LoRA merging raises NotImplementedError.
 """
 from __future__ import annotations
 
@@ -73,12 +73,15 @@ def load_pretrained_model(model_path, model_base=None, model_name="cambrian", lo
     """model/builder.py:29-175 for the LLaMA-family Cambrian checkpoints: returns (tokenizer, model, image_processor list,
     context_len).  `model_base` + `<model_path>/mm_projector.bin` is the connector-only layout (:103-114).
     load_4bit=True (:37-44): the checkpoint loads in bf16 on the CPU, the seven projections of every decoder layer are
-    quantised to NF4 layer by layer on `device` (quant.quantize_decoder_nf4_), everything else moves there in bf16."""
+    quantised to NF4 layer by layer on `device` (quant.quantize_decoder_nf4_), everything else moves there in bf16.
+    load_8bit=True (:35-36) does the same with LLM.int8 weights (quant_int8.quantize_decoder_int8_) and takes precedence
+    over load_4bit."""
     from transformers import AutoConfig, AutoTokenizer
 
     from .model.language_model.cambrian_llama import CambrianLlamaForCausalLM
-    if load_8bit:
-        raise NotImplementedError("8-bit (LLM.int8) loading is not supported; load_4bit=True gives NF4 decoder weights")
+    if load_8bit and torch.device(device).type == "cuda" and not torch.cuda.is_available():
+        # fail before the bf16 checkpoint is read into host memory: the int8 kernels exist for the GPU only
+        raise NotImplementedError("8-bit (LLM.int8) weights run on CUDA only and no CUDA device is available")
     if "lora" in model_name.lower():
         raise NotImplementedError("LoRA merging (builder.py:56-92) is outside the hot path: merge with the reference tools first")
     if "mistral" in model_name.lower() or "phi3" in model_name.lower():
@@ -91,7 +94,10 @@ def load_pretrained_model(model_path, model_base=None, model_name="cambrian", lo
         load_mm_projector(model, os.path.join(model_path, "mm_projector.bin"))
     else:
         model = CambrianLlamaForCausalLM.from_pretrained(model_path, torch_dtype=dtype, **kwargs)
-    if load_4bit:
+    if load_8bit:                                   # takes precedence over load_4bit, as in builder.py:35-38
+        from .quant_int8 import quantize_decoder_int8_
+        quantize_decoder_int8_(model, device)
+    elif load_4bit:
         from .quant import quantize_decoder_nf4_
         quantize_decoder_nf4_(model, device)
     model.to(device=device, dtype=dtype)

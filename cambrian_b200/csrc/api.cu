@@ -113,6 +113,12 @@ int gemv_nf4_launch(const void*, void*, int, int, int, long long, long long, int
                     cudaStream_t);
 int nf4_dequant_launch(void*, int, int, int, const int*, const void* const*, const void* const*, const void* const*,
                        const void* const*, cudaStream_t);
+int int8_quantize_weight_launch(const void*, int, int, long long, void*, float*, cudaStream_t);
+int int8_quantize_act_launch(const void*, int, int, long long, float, void*, float*, unsigned*, int*, int*, cudaStream_t);
+int gemv_int8_launch(const void*, const void*, const float*, const float*, const void*, long long, const int*, const int*,
+                     void*, int, int, int, long long, const void*, const void*, long long, int, cudaStream_t);
+int gemm_int8_launch(const void*, const void*, const float*, const float*, const void*, long long, const int*, const int*,
+                     void*, int, int, int, long long, const void*, const void*, long long, int, cudaStream_t);
 
 }  // namespace cb
 
@@ -362,6 +368,25 @@ int cb_gemv_nf4(const void* x, void* y, int M, int N, int K, int64_t ldx, int64_
 int cb_nf4_dequant(void* out, int N, int K, int nseg, const int32_t* seg_row0, const void* const* packed,
                    const void* const* qabsmax, const void* const* absmax2, const void* const* offset, void* stream) {
   return cb::nf4_dequant_launch(out, N, K, nseg, seg_row0, packed, qabsmax, absmax2, offset, ST(stream));
+}
+int cb_int8_quantize_weight(const void* w, int N, int K, int64_t ldw, void* cb, float* scb, void* stream) {
+  return cb::int8_quantize_weight_launch(w, N, K, ldw, cb, scb, ST(stream));
+}
+int cb_int8_quantize_act(const void* x, int M, int K, int64_t ldx, float threshold, void* xq, float* sca,
+                         uint32_t* colmax_ws, int32_t* outlier_idx, int32_t* n_outlier, void* stream) {
+  return cb::int8_quantize_act_launch(x, M, K, ldx, threshold, xq, sca, colmax_ws, outlier_idx, n_outlier, ST(stream));
+}
+int cb_gemv_int8(const void* xq, const void* cb, const float* sca, const float* scb, const void* x, int64_t ldx,
+                 const int32_t* outlier_idx, const int32_t* n_outlier, void* y, int M, int N, int K, int64_t ldy,
+                 const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream) {
+  return cb::gemv_int8_launch(xq, cb, sca, scb, x, ldx, outlier_idx, n_outlier, y, M, N, K, ldy, bias, residual, ldr,
+                              out_fp32, ST(stream));
+}
+int cb_gemm_int8(const void* xq, const void* cb, const float* sca, const float* scb, const void* x, int64_t ldx,
+                 const int32_t* outlier_idx, const int32_t* n_outlier, void* y, int M, int N, int K, int64_t ldy,
+                 const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream) {
+  return cb::gemm_int8_launch(xq, cb, sca, scb, x, ldx, outlier_idx, n_outlier, y, M, N, K, ldy, bias, residual, ldr,
+                              out_fp32, ST(stream));
 }
 
 }  // extern "C"

@@ -80,9 +80,10 @@ class TrainEngine:
                  background_optimizer: bool = False, collective: str = "nccl", offload_optimizer: bool = False):
         if zero_stage not in (0, 2):
             raise ValueError("zero_stage must be 0 or 2")
-        from .quant import is_quantized
-        if is_quantized(model):
-            raise ValueError("TrainEngine: the model has 4-bit (NF4) decoder weights, which are inference-only "
+        from .quant import quantized_format
+        fmt = quantized_format(model)
+        if fmt is not None:
+            raise ValueError(f"TrainEngine: the model has {fmt} decoder weights, which are inference-only "
                              "(QLoRA training is not supported)")
         if mm_projector_lr is not None and mm_vision_sampler_lr is not None:
             raise AssertionError("mm_projector_lr and mm_vision_sampler_lr are mutually exclusive")  # cambrian_trainer.py:259

@@ -159,6 +159,11 @@ class CBLlamaDecoderLayer(nn.Module):
         self.input_layernorm = CBRMSNorm(config.hidden_size, config.rms_norm_eps)
         self.post_attention_layernorm = CBRMSNorm(config.hidden_size, config.rms_norm_eps)
         self._nf4 = None        # NF4 projections (quant.quantize_decoder_nf4_): the bf16 weights are freed then
+        self._int8 = None       # LLM.int8 projections (quant_int8.quantize_decoder_int8_), likewise
+
+    def _quantized(self):
+        """{qkv, o, gate_up, down} -> projection objects with `linear(x, residual=None)` / `gate_up(x)`, or None."""
+        return self._nf4 if self._nf4 is not None else self._int8
 
     def _fused(self):
         a, m = self.self_attn, self.mlp
@@ -167,9 +172,10 @@ class CBLlamaDecoderLayer(nn.Module):
         return fuse_rows(qkv), fuse_rows(gu), _FusedGrad(qkv), _FusedGrad(gu)
 
     def forward(self, x, rt):
-        if self._nf4 is not None:
+        if self._quantized() is not None:
             if torch.is_grad_enabled():
-                raise NotImplementedError("a 4-bit (NF4) model is inference-only: training quantised weights (QLoRA) is "
+                fmt = "a 4-bit (NF4)" if self._nf4 is not None else "an 8-bit (LLM.int8)"
+                raise NotImplementedError(f"{fmt} model is inference-only: training quantised weights (QLoRA) is "
                                           "not supported; run it under torch.no_grad()")
             return self.infer(x, rt, None)
         a, m = self.self_attn, self.mlp
@@ -186,18 +192,18 @@ class CBLlamaDecoderLayer(nn.Module):
     @torch.no_grad()
     def infer(self, x, rt, cache):
         """KV-cache path (prefill and decode): same kernels, K/V appended to the per-layer cache.  cache=None: causal
-        attention over the sequence itself (no-grad forward of a 4-bit model).  NF4 layers run their projections through
-        ops.nf4_linear / ops.nf4_mlp_gate_up."""
+        attention over the sequence itself (no-grad forward of a quantised model).  Quantised layers (NF4 or int8) run
+        their projections through the format's projection objects (`linear` / `gate_up`)."""
         a, m = self.self_attn, self.mlp
-        nf4 = self._nf4
-        if nf4 is None:
+        qp = self._quantized()
+        if qp is None:
             qkv_w, gu_w, _, _ = self._fused()
         B, S, H = x.shape
         nh, nkv, hd = self.nh, self.nkv, self.hd
         rows = B * S
         x2 = x.reshape(rows, H)
         h = ops.rmsnorm_fwd(x2, self.input_layernorm.weight, self.input_layernorm.variance_epsilon, rt["hf_cast"])
-        qkv = ops.nf4_linear(h, nf4["qkv"]) if nf4 is not None else ops.gemm(h, qkv_w)
+        qkv = qp["qkv"].linear(h) if qp is not None else ops.gemm(h, qkv_w)
         ops.rope_(qkv, rt["pos"], rt["cos"], rt["sin"], nh + nkv, hd)
         q = qkv[:, : nh * hd].view(B, S, nh, hd)
         k_new = qkv[:, nh * hd:(nh + nkv) * hd].view(B, S, nkv, hd)
@@ -218,15 +224,15 @@ class CBLlamaDecoderLayer(nn.Module):
             vc[:, t0:t0 + S].copy_(v_new)
             attn = ops.attn_fwd(q, kc[:, : t0 + S], vc[:, : t0 + S], causal=True, kmask=rt["kmask"])
         attn2 = attn.view(rows, nh * hd)
-        if nf4 is not None:
-            x1 = ops.nf4_linear(attn2, nf4["o"], residual=x2)
+        if qp is not None:
+            x1 = qp["o"].linear(attn2, residual=x2)
         else:
             x1 = ops.gemm(attn2, a.o_proj.weight, residual=x2)
         h2 = ops.rmsnorm_fwd(x1, self.post_attention_layernorm.weight, self.post_attention_layernorm.variance_epsilon,
                              rt["hf_cast"])
-        if nf4 is not None:
-            _, act = ops.nf4_mlp_gate_up(h2, nf4["gate_up"])
-            return ops.nf4_linear(act, nf4["down"], residual=x1).view(B, S, H)
+        if qp is not None:
+            _, act = qp["gate_up"].gate_up(h2)
+            return qp["down"].linear(act, residual=x1).view(B, S, H)
         _, act = ops.mlp_gate_up(h2, gu_w)
         return ops.gemm(act, m.down_proj.weight, residual=x1).view(B, S, H)
 
@@ -430,9 +436,10 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
         return self.model
 
     def save_pretrained(self, *args, **kwargs):
-        from ...quant import is_quantized
-        if is_quantized(self):
-            raise NotImplementedError("save_pretrained of a 4-bit (NF4) model is not supported: its decoder projections "
+        from ...quant import quantized_format
+        fmt = quantized_format(self)
+        if fmt is not None:
+            raise NotImplementedError(f"save_pretrained of a {fmt} model is not supported: its decoder projections "
                                       "hold no bf16 weights; save the bf16 checkpoint it was loaded from instead")
         return super().save_pretrained(*args, **kwargs)
 

@@ -792,3 +792,80 @@ def nf4_mlp_gate_up(h2d, qw):
         I = qw.N // 2
         return gu, swiglu_fwd(gu[:, :I], gu[:, I:])
     return mlp_gate_up(h2d, nf4_dequant(qw))
+
+
+# ------------------------------------------------------------------------------------------------
+# LLM.int8 decoder weights (load_8bit; the format and the epilogue order live in quant_int8.py)
+# ------------------------------------------------------------------------------------------------
+def int8_quantize_weight(w, cb, scb):
+    """Quantise one bf16 [N, K] weight (contiguous rows) into caller-allocated cb int8 [N, K] and scb fp32 [N]."""
+    _require_cuda_bf16(w)
+    N, K = w.shape
+    if w.stride(1) != 1 or cb.shape != (N, K) or not cb.is_contiguous() or scb.shape != (N,) or scb.dtype != torch.float32:
+        raise ValueError("int8_quantize_weight: need w [N, K] with contiguous rows, cb int8 [N, K], scb fp32 [N]")
+    check(_lib.load().cb_int8_quantize_weight(ptr(w), N, K, w.stride(0), ptr(cb), ptr(scb), stream()),
+          "cb_int8_quantize_weight")
+
+
+def int8_quantize_act(x, threshold: float):
+    """x [M, K] bf16 -> (xq int8 [M, K], sca fp32 [M], outlier_idx int32 [K] (first n_outlier used, ascending),
+    n_outlier int32 [1]); all on the device, no host sync."""
+    _require_cuda_bf16(x)
+    M, K = x.shape
+    if x.stride(1) != 1:
+        raise ValueError("int8_quantize_act: x must have contiguous rows")
+    dev = x.device
+    xq = torch.empty((M, K), dtype=torch.int8, device=dev)
+    sca = torch.empty(M, dtype=torch.float32, device=dev)
+    colmax = torch.empty(K, dtype=torch.int32, device=dev)
+    idx = torch.empty(K, dtype=torch.int32, device=dev)
+    cnt = torch.empty(1, dtype=torch.int32, device=dev)
+    check(_lib.load().cb_int8_quantize_act(ptr(x), M, K, x.stride(0), float(threshold), ptr(xq), ptr(sca), ptr(colmax),
+                                           ptr(idx), ptr(cnt), stream()), "cb_int8_quantize_act")
+    return xq, sca, idx, cnt
+
+
+def _int8_matmul(entry, x, qa, qw, bias, residual, out, out_dtype):
+    _require_cuda_bf16(x, bias, residual)
+    xq, sca, idx, cnt = qa
+    M, K = xq.shape
+    N = qw.N
+    if K != qw.K or x.shape != (M, K) or x.stride(1) != 1:
+        raise ValueError(f"{entry}: activation {tuple(x.shape)} does not match K = {qw.K}")
+    if out is None:
+        out = torch.empty((M, N), dtype=out_dtype, device=x.device)
+    if out.dtype not in (torch.bfloat16, torch.float32) or out.stride(-1) != 1 or out.shape != (M, N):
+        raise ValueError(f"{entry}: out must be a bf16 / fp32 [M, N] tensor with contiguous rows")
+    if residual is not None and (residual.shape != out.shape or residual.stride(-1) != 1):
+        raise ValueError(f"{entry}: residual must match the output shape")
+    check(getattr(_lib.load(), entry)(ptr(xq), ptr(qw.w.cb), ptr(sca), ptr(qw.w.scb), ptr(x), x.stride(0), ptr(idx),
+                                      ptr(cnt), ptr(out), M, N, K, out.stride(0), ptr(bias), ptr(residual),
+                                      residual.stride(0) if residual is not None else 0, int(out.dtype == torch.float32),
+                                      stream()), entry)
+    return out
+
+
+def gemv_int8(x, qa, qw, bias=None, residual=None, out=None, out_dtype=torch.bfloat16) -> torch.Tensor:
+    """y[M, N] for M <= 8 rows (decode) from x, its quantisation qa = int8_quantize_act(x) and an Int8Projection."""
+    return _int8_matmul("cb_gemv_int8", x, qa, qw, bias, residual, out, out_dtype)
+
+
+def gemm_int8(x, qa, qw, bias=None, residual=None, out=None, out_dtype=torch.bfloat16) -> torch.Tensor:
+    """The same product on the int8 tensor cores, any M (prefill, batches above 8 rows)."""
+    return _int8_matmul("cb_gemm_int8", x, qa, qw, bias, residual, out, out_dtype)
+
+
+def int8_linear(x, qw, residual=None, out=None, out_dtype=torch.bfloat16) -> torch.Tensor:
+    """y = x @ W^T (+ residual) on an int8 projection (quant_int8.Int8Projection): the activation is quantised with the
+    projection's outlier threshold, then M <= 8 rows run the dp4a GEMV and larger M the int8 tensor-core GEMM."""
+    qa = int8_quantize_act(x, qw.threshold)
+    if x.shape[0] <= 8:
+        return gemv_int8(x, qa, qw, residual=residual, out=out, out_dtype=out_dtype)
+    return gemm_int8(x, qa, qw, residual=residual, out=out, out_dtype=out_dtype)
+
+
+def int8_mlp_gate_up(h2d, qw):
+    """`mlp_gate_up` on the stacked int8 gate|up projection: (gu [M, 2F], act = silu(gate) * up)."""
+    gu = int8_linear(h2d, qw)
+    I = qw.N // 2
+    return gu, swiglu_fwd(gu[:, :I], gu[:, I:])

@@ -70,6 +70,14 @@ class NF4Projection:
         self.row0 = [sum(p.shape[0] for p in parts[:i]) for i in range(len(parts))]
         self.scratch = scratch
 
+    def linear(self, x, residual=None):
+        from . import ops
+        return ops.nf4_linear(x, self, residual=residual)
+
+    def gate_up(self, x):
+        from . import ops
+        return ops.nf4_mlp_gate_up(x, self)
+
     def segment_arrays(self):
         return self.row0, [p.packed for p in self.parts], [p.qabsmax for p in self.parts], \
             [p.absmax2 for p in self.parts], [p.offset for p in self.parts]
@@ -101,9 +109,20 @@ def quantize(w: torch.Tensor, workspace: torch.Tensor | None = None) -> NF4Weigh
     return qw
 
 
+def quantized_format(model) -> str | None:
+    """"4-bit (NF4)" or "8-bit (LLM.int8)" when a decoder layer of `model` carries quantised weights
+    (quantize_decoder_nf4_ / quant_int8.quantize_decoder_int8_), else None: the wording of every refusal."""
+    for m in model.modules():
+        if getattr(m, "_nf4", None) is not None:
+            return "4-bit (NF4)"
+        if getattr(m, "_int8", None) is not None:
+            return "8-bit (LLM.int8)"
+    return None
+
+
 def is_quantized(model) -> bool:
-    """True when any decoder layer of `model` carries NF4 weights (quantize_decoder_nf4_)."""
-    return any(getattr(m, "_nf4", None) is not None for m in model.modules())
+    """True when any decoder layer of `model` carries NF4 or int8 weights."""
+    return quantized_format(model) is not None
 
 
 @torch.no_grad()

@@ -28,9 +28,11 @@ class Zero3Inference:
     def __init__(self, model, process_group=None):
         """`model`: a CambrianLlamaForCausalLM already on its device in bf16 (full weights are dropped layer by layer
         as they are sharded; load on CPU / meta and move layer-wise for models that do not fit one GPU)."""
-        from .quant import is_quantized
-        if is_quantized(model):
-            raise ValueError("Zero3Inference: 4-bit (NF4) decoder layers are not sharded; a 4-bit model runs on one GPU")
+        from .quant import quantized_format
+        fmt = quantized_format(model)
+        if fmt is not None:
+            raise ValueError(f"Zero3Inference: {fmt} decoder layers are not sharded; a {fmt.split()[0]} model runs on "
+                             "one GPU")
         self.pg = process_group
         self.world = dist.get_world_size(process_group) if dist.is_available() and dist.is_initialized() else 1
         self.rank = dist.get_rank(process_group) if self.world > 1 else 0

@@ -278,6 +278,30 @@ int cb_gemv_nf4(const void* x, void* y, int M, int N, int K, int64_t ldx, int64_
  * bitwise equal to the definition above: the larger-batch path runs the bf16 GEMM on it. */
 int cb_nf4_dequant(void* out, int N, int K, int nseg, const int32_t* seg_row0, const void* const* packed,
                    const void* const* qabsmax, const void* const* absmax2, const void* const* offset, void* stream);
+/* 8-bit LLM.int8 decoder weights, the `load_8bit` path of model/builder.py:35-36 (bitsandbytes LLM.int8 with
+ * llm_int8_threshold = 6.0 there; the format and the exact order of the epilogue are defined in
+ * cambrian_b200/quant_int8.py).  Per-row absmax scales on both sides, K % 16 == 0:
+ *   weight:     scb[n] = max |W[n,:]|, cb[n,k] = clamp(rint(W[n,k] * (127 / scb[n])), -127, 127), int8 [N, K];
+ *   activation: outlier columns O = { j : max_m |x[m,j]| >= threshold } (none when threshold <= 0), sca[m] = max |x[m,j]|
+ *               over j not in O, xq[m,j] = rint(x[m,j] * (127 / sca[m])) off O and 0 on O, int8 [M, K];
+ *   output:     y = (float(sum xq cb) * (sca * scb)) * (1/16129) + sum_{j in O, ascending} x[m,j] * (float(cb[n,j]) *
+ *               (scb[n] * (1/127))) (+ bias[n]) (+ residual[m,n]), every operation rounded on its own (no FMA).
+ *
+ * cb_int8_quantize_weight: one bf16 W [N, K] (row stride ldw) -> cb (row stride K), scb; deterministic, no host sync. */
+int cb_int8_quantize_weight(const void* w, int N, int K, int64_t ldw, void* cb, float* scb, void* stream);
+/* x [M, K] bf16 (row stride ldx) -> xq [M, K] int8, sca [M] fp32, outlier_idx [<= K] int32 ascending, n_outlier [1]
+ * int32 on the device; colmax_ws is caller-provided scratch of K uint32.  No host synchronisation (graph-capturable). */
+int cb_int8_quantize_act(const void* x, int M, int K, int64_t ldx, float threshold, void* xq, float* sca,
+                         uint32_t* colmax_ws, int32_t* outlier_idx, int32_t* n_outlier, void* stream);
+/* y[M,N] (bf16 or fp32, row stride ldy) from the quantised activation (xq, sca, outliers; x is the bf16 activation it
+ * came from) and weight (cb, scb) — M <= 8 rows (decode): CUDA-core dp4a GEMV; any M: int8 tensor-core GEMM
+ * (wgmma .s32.s8.s8).  Both are bitwise equal to the definition above, so to each other. */
+int cb_gemv_int8(const void* xq, const void* cb, const float* sca, const float* scb, const void* x, int64_t ldx,
+                 const int32_t* outlier_idx, const int32_t* n_outlier, void* y, int M, int N, int K, int64_t ldy,
+                 const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream);
+int cb_gemm_int8(const void* xq, const void* cb, const float* sca, const float* scb, const void* x, int64_t ldx,
+                 const int32_t* outlier_idx, const int32_t* n_outlier, void* y, int M, int N, int K, int64_t ldy,
+                 const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,10 +1,11 @@
 """Single-GPU decode latency of the Cambrian-8B-shaped model (A12): ms/token of the KV-cache greedy loop after a multimodal
 prefill, against the weight-streaming floor (bf16 weights / measured HBM bandwidth).
 
-    python tools/decode_bench.py [--batch 1] [--prompt 1024] [--new 64] [--config 8b-ddp | yi34b] [--load-4bit]
+    python tools/decode_bench.py [--batch 1] [--prompt 1024] [--new 64] [--config 8b-ddp | yi34b] [--load-4bit | --load-8bit]
 
---load-4bit quantises the decoder projections to NF4 (cambrian_b200/quant.py) layer by layer after building the model on
-the CPU, so configurations whose bf16 decoder does not fit one GPU (--config yi34b: Cambrian-34B-shaped, 60 layers) run.
+--load-4bit quantises the decoder projections to NF4 (cambrian_b200/quant.py), --load-8bit to LLM.int8
+(cambrian_b200/quant_int8.py), layer by layer after building the model on the CPU, so configurations whose bf16 decoder
+does not fit one GPU (--config yi34b: Cambrian-34B-shaped, 60 layers) run.  8-bit takes precedence, as in the loader.
 """
 import argparse
 import json
@@ -28,9 +29,10 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="eager per-token loop instead of the CUDA-graph replay")
     ap.add_argument("--profile", action="store_true", help="kernel time per token by kernel name (torch.profiler)")
     ap.add_argument("--load-4bit", action="store_true", help="NF4 decoder projections (quant.quantize_decoder_nf4_)")
+    ap.add_argument("--load-8bit", action="store_true", help="LLM.int8 decoder projections (quant_int8)")
     ap.add_argument("--layers", type=int, default=60, help="decoder layers of --config yi34b")
     args = ap.parse_args()
-    from cambrian_b200 import quant
+    from cambrian_b200 import quant, quant_int8
     from cambrian_b200.model.language_model.cambrian_llama import CambrianLlamaForCausalLM
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(0)
@@ -45,10 +47,12 @@ def main():
     prev = torch.get_default_dtype()
     torch.set_default_dtype(torch.bfloat16)
     qstats = None
-    if args.load_4bit and args.config == "yi34b":
+    quantize = (quant_int8.quantize_decoder_int8_ if args.load_8bit else
+                quant.quantize_decoder_nf4_ if args.load_4bit else None)
+    if quantize is not None and args.config == "yi34b":
         # built on the CPU (a 34B decoder does not fit the GPU in bf16), quantised onto the GPU one layer at a time
         model = CambrianLlamaForCausalLM(cfg)
-        qstats = quant.quantize_decoder_nf4_(model, dev)
+        qstats = quantize(model, dev)
         model.to(dev)
         with torch.device(dev):
             for t in model.get_model().vision_tower_aux_list:
@@ -58,8 +62,8 @@ def main():
             model = CambrianLlamaForCausalLM(cfg)
             for t in model.get_model().vision_tower_aux_list:
                 t.load_model()
-        if args.load_4bit:
-            qstats = quant.quantize_decoder_nf4_(model, dev)
+        if quantize is not None:
+            qstats = quantize(model, dev)
             torch.cuda.empty_cache()
     torch.set_default_dtype(prev)
     model.eval()
@@ -92,11 +96,12 @@ def one_batch(args, model, cfg, dev, B):
     t1, l1, _ = run(1)
     tn, ln, out = run(args.new + 1)
     ms_tok = (tn - t1) / args.new
-    # weight bytes one decode step streams: decoder layers (bf16 or NF4) + norms + lm_head
+    # weight bytes one decode step streams: decoder layers (bf16, NF4 or int8) + norms + lm_head
     qstats = model._bench_qstats
     n_params = sum(p.numel() for n, p in model.named_parameters() if "vision" not in n and "mm_projector" not in n
                    and "embed_tokens" not in n)
-    weight_bytes = n_params * 2 + (qstats["nf4_bytes"] if qstats else 0)
+    q_bytes = (qstats.get("nf4_bytes") or qstats.get("int8_bytes")) if qstats else None
+    weight_bytes = n_params * 2 + (q_bytes or 0)
     hbm = bench.peaks()[0]
     floor = weight_bytes / (hbm * 1e9) * 1e3
     top = None
@@ -112,13 +117,15 @@ def one_batch(args, model, cfg, dev, B):
                 a_[1] += 1
         top = [dict(kernel=k, ms_per_token=round(v[0] / 1e3 / args.new, 4), launches_per_token=round(v[1] / args.new, 1))
                for k, v in sorted(agg.items(), key=lambda kv: -kv[1][0])[:14]]
-    print(json.dumps(dict(metric="decode_ms_per_token", value=ms_tok, unit="ms", config=args.config, load_4bit=args.load_4bit,
+    print(json.dumps(dict(metric="decode_ms_per_token", value=ms_tok, unit="ms", config=args.config, load_4bit=args.load_4bit and not args.load_8bit,
+                          load_8bit=args.load_8bit,
                           batch=B, prompt=args.prompt, new_tokens=args.new, prefill_ms=t1, tokens_per_s=B * 1000.0 / ms_tok,
                           launches_per_token=(ln - l1) / args.new, decode_graph=not args.no_graph, weight_bytes=weight_bytes,
-                          decoder_nf4_bytes=qstats["nf4_bytes"] if qstats else None,
+                          decoder_nf4_bytes=qstats.get("nf4_bytes") if qstats else None,
+                          decoder_int8_bytes=qstats.get("int8_bytes") if qstats else None,
                           peak_mem_gb=torch.cuda.max_memory_allocated() / 2 ** 30, gpu=torch.cuda.get_device_name(0),
                           floor_ms=floor, frac_of_floor=floor / ms_tok,
-                          note="floor = weight bytes per step (decoder bf16 or NF4, lm_head bf16) / measured HBM copy "
+                          note="floor = weight bytes per step (decoder bf16, NF4 or int8, lm_head bf16) / measured HBM copy "
                                "bandwidth", top_kernels=top)),
           flush=True)
 
