@@ -83,6 +83,10 @@ SIGNATURES = {
     "cb_int8_quantize_act": (_i, [_vp, _i, _i, _i64, _f, _vp, _vp, _vp, _vp, _vp, _vp]),
     "cb_gemv_int8": (_i, [_vp] * 5 + [_i64, _vp, _vp, _vp, _i, _i, _i, _i64, _vp, _vp, _i64, _i, _vp]),
     "cb_gemm_int8": (_i, [_vp] * 5 + [_i64, _vp, _vp, _vp, _i, _i, _i, _i64, _vp, _vp, _i64, _i, _vp]),
+    "cb_fp8_quantize_weight": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp]),
+    "cb_fp8_quantize_act": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp]),
+    "cb_gemv_fp8": (_i, [_vp] * 5 + [_i, _i, _i, _i64, _vp, _vp, _i64, _i, _vp]),
+    "cb_gemm_fp8": (_i, [_vp] * 5 + [_i, _i, _i, _i64, _vp, _vp, _i64, _i, _vp]),
 }
 
 _lib = None

@@ -10,7 +10,7 @@ the unchanged `PreTrainedModel.from_pretrained`.  This file adds the three refer
     `pretrain_mm_mlp_adapter` path of `initialize_vision_modules` (cambrian_arch.py:183-200, strict per sub-module);
   * `load_pretrained_model` — the loader the eval / serve harness calls (model/builder.py:29-175), bf16 on one GPU, or
     with `load_4bit=True` the decoder projections in NF4 (quant.py), with `load_8bit=True` in LLM.int8
-    (quant_int8.py).  LoRA merging raises NotImplementedError.
+    (quant_int8.py), with `load_fp8=True` in FP8 E4M3 (quant_fp8.py).  LoRA merging raises NotImplementedError.
 """
 from __future__ import annotations
 
@@ -69,16 +69,22 @@ def load_mm_projector(model, path_or_state, strict_submodules: bool = False):
 
 
 def load_pretrained_model(model_path, model_base=None, model_name="cambrian", load_8bit=False, load_4bit=False,
-                          device="cuda", dtype=torch.bfloat16, load_tokenizer=True, **kwargs):
+                          device="cuda", dtype=torch.bfloat16, load_tokenizer=True, load_fp8=False, **kwargs):
     """model/builder.py:29-175 for the LLaMA-family Cambrian checkpoints: returns (tokenizer, model, image_processor list,
     context_len).  `model_base` + `<model_path>/mm_projector.bin` is the connector-only layout (:103-114).
     load_4bit=True (:37-44): the checkpoint loads in bf16 on the CPU, the seven projections of every decoder layer are
     quantised to NF4 layer by layer on `device` (quant.quantize_decoder_nf4_), everything else moves there in bf16.
     load_8bit=True (:35-36) does the same with LLM.int8 weights (quant_int8.quantize_decoder_int8_) and takes precedence
-    over load_4bit."""
+    over load_4bit.  load_fp8=True (no reference counterpart) does the same with FP8 E4M3 weights
+    (quant_fp8.quantize_decoder_fp8_); it names one format, so combining it with load_4bit or load_8bit is a ValueError."""
     from transformers import AutoConfig, AutoTokenizer
 
     from .model.language_model.cambrian_llama import CambrianLlamaForCausalLM
+    if load_fp8 and (load_4bit or load_8bit):
+        raise ValueError("load_fp8 cannot be combined with load_4bit or load_8bit: choose one weight format")
+    if load_fp8 and torch.device(device).type == "cuda" and not torch.cuda.is_available():
+        # fail before the bf16 checkpoint is read into host memory: the FP8 kernels exist for the GPU only
+        raise NotImplementedError("8-bit (FP8) weights run on CUDA only and no CUDA device is available")
     if load_8bit and torch.device(device).type == "cuda" and not torch.cuda.is_available():
         # fail before the bf16 checkpoint is read into host memory: the int8 kernels exist for the GPU only
         raise NotImplementedError("8-bit (LLM.int8) weights run on CUDA only and no CUDA device is available")
@@ -94,7 +100,10 @@ def load_pretrained_model(model_path, model_base=None, model_name="cambrian", lo
         load_mm_projector(model, os.path.join(model_path, "mm_projector.bin"))
     else:
         model = CambrianLlamaForCausalLM.from_pretrained(model_path, torch_dtype=dtype, **kwargs)
-    if load_8bit:                                   # takes precedence over load_4bit, as in builder.py:35-38
+    if load_fp8:
+        from .quant_fp8 import quantize_decoder_fp8_
+        quantize_decoder_fp8_(model, device)
+    elif load_8bit:                                 # takes precedence over load_4bit, as in builder.py:35-38
         from .quant_int8 import quantize_decoder_int8_
         quantize_decoder_int8_(model, device)
     elif load_4bit:

@@ -119,6 +119,12 @@ int gemv_int8_launch(const void*, const void*, const float*, const float*, const
                      void*, int, int, int, long long, const void*, const void*, long long, int, cudaStream_t);
 int gemm_int8_launch(const void*, const void*, const float*, const float*, const void*, long long, const int*, const int*,
                      void*, int, int, int, long long, const void*, const void*, long long, int, cudaStream_t);
+int fp8_quantize_weight_launch(const void*, int, int, long long, void*, float*, cudaStream_t);
+int fp8_quantize_act_launch(const void*, int, int, long long, void*, float*, cudaStream_t);
+int gemv_fp8_launch(const void*, const void*, const float*, const float*, void*, int, int, int, long long, const void*,
+                    const void*, long long, int, cudaStream_t);
+int gemm_fp8_launch(const void*, const void*, const float*, const float*, void*, int, int, int, long long, const void*,
+                    const void*, long long, int, cudaStream_t);
 
 }  // namespace cb
 
@@ -387,6 +393,20 @@ int cb_gemm_int8(const void* xq, const void* cb, const float* sca, const float* 
                  const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream) {
   return cb::gemm_int8_launch(xq, cb, sca, scb, x, ldx, outlier_idx, n_outlier, y, M, N, K, ldy, bias, residual, ldr,
                               out_fp32, ST(stream));
+}
+int cb_fp8_quantize_weight(const void* w, int N, int K, int64_t ldw, void* wq, float* sw, void* stream) {
+  return cb::fp8_quantize_weight_launch(w, N, K, ldw, wq, sw, ST(stream));
+}
+int cb_fp8_quantize_act(const void* x, int M, int K, int64_t ldx, void* xq, float* sa, void* stream) {
+  return cb::fp8_quantize_act_launch(x, M, K, ldx, xq, sa, ST(stream));
+}
+int cb_gemv_fp8(const void* xq, const void* wq, const float* sa, const float* sw, void* y, int M, int N, int K,
+                int64_t ldy, const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream) {
+  return cb::gemv_fp8_launch(xq, wq, sa, sw, y, M, N, K, ldy, bias, residual, ldr, out_fp32, ST(stream));
+}
+int cb_gemm_fp8(const void* xq, const void* wq, const float* sa, const float* sw, void* y, int M, int N, int K,
+                int64_t ldy, const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream) {
+  return cb::gemm_fp8_launch(xq, wq, sa, sw, y, M, N, K, ldy, bias, residual, ldr, out_fp32, ST(stream));
 }
 
 }  // extern "C"

@@ -14,11 +14,9 @@
 //   i8_quant_act_kernel                             cb_int8_quantize_act, three stream-ordered passes, no host sync
 //   gemv_int8_kernel<M>                             decode projections, M <= 8 rows (cb_gemv_int8): dp4a
 //   gemm_int8_wgmma                                 M > 8 (cb_gemm_int8): TMA ring + wgmma m64n128k32 .s32.s8.s8
-#include "common.cuh"
+#include "bytegemm.cuh"
 #include <algorithm>
 #include <cstring>
-#include <cudaTypedefs.h>
-#include <mutex>
 
 namespace cb {
 
@@ -302,26 +300,13 @@ __global__ void __launch_bounds__(IG_WARPS * 32) gemv_int8_kernel(const int8_t* 
 // descriptor start each) with one k-block group in flight.  The epilogue works from the s32 registers: the int8 term
 // per element, then the outlier term read from L2 (x[m, O] and cb[n, O]), then bias / residual and the store.
 // ---------------------------------------------------------------------------------------------------------------------
-constexpr int QBM = 128, QBN = 128, QBK = 128;
 constexpr int Q_STAGES = 6;
-constexpr int Q_A_BYTES = QBM * QBK, Q_B_BYTES = QBN * QBK, Q_STAGE_BYTES = Q_A_BYTES + Q_B_BYTES;
 constexpr int Q_SMEM_BYTES = Q_STAGES * Q_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 static_assert(Q_SMEM_BYTES <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
-constexpr int Q_GROUP_M = 16;
 
 __device__ __forceinline__ void i8_reg_fence(int32_t (&d)[64]) {
 #pragma unroll
   for (int i = 0; i < 64; ++i) asm volatile("" : "+r"(d[i])::"memory");
-}
-
-__device__ __forceinline__ void i8_tile_to_mn(int r, int m_blocks, int n_blocks, int& mb, int& nb) {
-  const int tpg = Q_GROUP_M * n_blocks;
-  const int g = r / tpg;
-  const int first = g * Q_GROUP_M;
-  const int gs = min(Q_GROUP_M, m_blocks - first);
-  const int w = r - g * tpg;
-  mb = first + w % gs;
-  nb = w / gs;
 }
 
 __global__ void __launch_bounds__(288, 1)
@@ -350,25 +335,7 @@ gemm_int8_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   __syncthreads();
 
   if (warp == 8) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int r = blockIdx.x; r < tiles; r += gridDim.x) {
-        int mb, nb;
-        i8_tile_to_mn(r, m_blocks, n_blocks, mb, nb);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
-          const uint32_t sa = smem_base + stage * Q_STAGE_BYTES;
-          mbar_arrive_expect_tx(full_bar(stage), Q_STAGE_BYTES);
-          tma_load_3d(sa, &tmA, full_bar(stage), kb * QBK, mb * QBM, 0);
-          tma_load_3d(sa + Q_A_BYTES, &tmB, full_bar(stage), kb * QBK, nb * QBN, 0);
-          if (++stage == Q_STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-      }
-    }
+    if (lane == 0) q_produce<Q_STAGES>(&tmA, &tmB, smem_base, bar_base, M, N, K, tiles);
     return;
   }
 
@@ -382,7 +349,7 @@ gemm_int8_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   uint32_t phase = 0;
   for (int r = blockIdx.x; r < tiles; r += gridDim.x) {
     int mb, nb;
-    i8_tile_to_mn(r, m_blocks, n_blocks, mb, nb);
+    q_tile_to_mn(r, m_blocks, n_blocks, mb, nb);
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0;
     int prev_stage = -1;
@@ -457,39 +424,6 @@ gemm_int8_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 // ---------------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------------
-static PFN_cuTensorMapEncodeTiled_v12000 i8_encode_fn() {
-  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(p);
-  });
-  return fn;
-}
-
-// int8 [rows, K] row-major (row stride K bytes), box 128 (K) x 128 rows, SWIZZLE_128B; out-of-range elements read as 0
-static int make_tmap_i8(CUtensorMap* out, const void* base, uint64_t K, uint64_t rows) {
-  auto fn = i8_encode_fn();
-  if (!fn) return set_error(CB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t dims[3] = {K, rows, 1};
-  cuuint64_t strides[2] = {K, K * rows};
-  cuuint32_t box[3] = {QBK, 128, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = CUDA_SUCCESS;
-  for (int attempt = 0; attempt < 2; ++attempt) {
-    r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(base), dims, strides, box, estr,
-           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_ERROR_INVALID_CONTEXT) break;
-    cudaFree(0);  // a thread with no driver context bound yet: bind the primary context and retry
-  }
-  if (r != CUDA_SUCCESS) return set_error(CB_ERR_CUDA, "cuTensorMapEncodeTiled (int8) failed (%d)", (int)r);
-  return CB_OK;
-}
-
 static int i8_epi(I8Epi& ep, const char* who, int M, int N, int K, const void* xq, const void* cb, const float* sca,
                   const float* scb, const void* x, long long ldx, const int* oidx, const int* ocnt, void* y,
                   long long ldy, const void* bias, const void* residual, long long ldr, int out_fp32) {
@@ -538,8 +472,8 @@ int gemm_int8_launch(const void* xq, const void* cb, const float* sca, const flo
   int rc = i8_epi(ep, "gemm_int8", M, N, K, xq, cb, sca, scb, x, ldx, oidx, ocnt, y, ldy, bias, residual, ldr, out_fp32);
   if (rc != CB_OK) return rc;
   CUtensorMap ta, tb;
-  if ((rc = make_tmap_i8(&ta, xq, K, M))) return rc;
-  if ((rc = make_tmap_i8(&tb, cb, K, N))) return rc;
+  if ((rc = make_tmap_u8(&ta, xq, K, M, QBM))) return rc;
+  if ((rc = make_tmap_u8(&tb, cb, K, N, QBN))) return rc;
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(gemm_int8_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, Q_SMEM_BYTES);

@@ -160,10 +160,11 @@ class CBLlamaDecoderLayer(nn.Module):
         self.post_attention_layernorm = CBRMSNorm(config.hidden_size, config.rms_norm_eps)
         self._nf4 = None        # NF4 projections (quant.quantize_decoder_nf4_): the bf16 weights are freed then
         self._int8 = None       # LLM.int8 projections (quant_int8.quantize_decoder_int8_), likewise
+        self._fp8 = None        # FP8 E4M3 projections (quant_fp8.quantize_decoder_fp8_), likewise
 
     def _quantized(self):
         """{qkv, o, gate_up, down} -> projection objects with `linear(x, residual=None)` / `gate_up(x)`, or None."""
-        return self._nf4 if self._nf4 is not None else self._int8
+        return next((q for q in (self._nf4, self._int8, self._fp8) if q is not None), None)
 
     def _fused(self):
         a, m = self.self_attn, self.mlp
@@ -174,7 +175,8 @@ class CBLlamaDecoderLayer(nn.Module):
     def forward(self, x, rt):
         if self._quantized() is not None:
             if torch.is_grad_enabled():
-                fmt = "a 4-bit (NF4)" if self._nf4 is not None else "an 8-bit (LLM.int8)"
+                fmt = ("a 4-bit (NF4)" if self._nf4 is not None else
+                       "an 8-bit (LLM.int8)" if self._int8 is not None else "an 8-bit (FP8)")
                 raise NotImplementedError(f"{fmt} model is inference-only: training quantised weights (QLoRA) is "
                                           "not supported; run it under torch.no_grad()")
             return self.infer(x, rt, None)
@@ -192,7 +194,7 @@ class CBLlamaDecoderLayer(nn.Module):
     @torch.no_grad()
     def infer(self, x, rt, cache):
         """KV-cache path (prefill and decode): same kernels, K/V appended to the per-layer cache.  cache=None: causal
-        attention over the sequence itself (no-grad forward of a quantised model).  Quantised layers (NF4 or int8) run
+        attention over the sequence itself (no-grad forward of a quantised model).  Quantised layers (NF4, int8 or FP8) run
         their projections through the format's projection objects (`linear` / `gate_up`)."""
         a, m = self.self_attn, self.mlp
         qp = self._quantized()

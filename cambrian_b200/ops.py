@@ -869,3 +869,74 @@ def int8_mlp_gate_up(h2d, qw):
     gu = int8_linear(h2d, qw)
     I = qw.N // 2
     return gu, swiglu_fwd(gu[:, :I], gu[:, I:])
+
+
+# ------------------------------------------------------------------------------------------------
+# FP8 E4M3 decoder weights (load_fp8; the format and the epilogue order live in quant_fp8.py)
+# ------------------------------------------------------------------------------------------------
+def fp8_quantize_weight(w, wq, sw):
+    """Quantise one bf16 [N, K] weight (contiguous rows) into caller-allocated wq float8_e4m3fn [N, K] and sw fp32 [N]."""
+    _require_cuda_bf16(w)
+    N, K = w.shape
+    if (w.stride(1) != 1 or wq.shape != (N, K) or not wq.is_contiguous() or wq.dtype != torch.float8_e4m3fn
+            or sw.shape != (N,) or sw.dtype != torch.float32):
+        raise ValueError("fp8_quantize_weight: need w [N, K] with contiguous rows, wq float8_e4m3fn [N, K], sw fp32 [N]")
+    check(_lib.load().cb_fp8_quantize_weight(ptr(w), N, K, w.stride(0), ptr(wq), ptr(sw), stream()),
+          "cb_fp8_quantize_weight")
+
+
+def fp8_quantize_act(x):
+    """x [M, K] bf16 -> (xq float8_e4m3fn [M, K], sa fp32 [M]) on the device, no host sync."""
+    _require_cuda_bf16(x)
+    M, K = x.shape
+    if x.stride(1) != 1:
+        raise ValueError("fp8_quantize_act: x must have contiguous rows")
+    xq = torch.empty((M, K), dtype=torch.float8_e4m3fn, device=x.device)
+    sa = torch.empty(M, dtype=torch.float32, device=x.device)
+    check(_lib.load().cb_fp8_quantize_act(ptr(x), M, K, x.stride(0), ptr(xq), ptr(sa), stream()), "cb_fp8_quantize_act")
+    return xq, sa
+
+
+def _fp8_matmul(entry, qa, qw, bias, residual, out, out_dtype):
+    _require_cuda_bf16(bias, residual)
+    xq, sa = qa
+    M, K = xq.shape
+    N = qw.N
+    if K != qw.K or xq.dtype != torch.float8_e4m3fn or not xq.is_contiguous() or sa.shape != (M,):
+        raise ValueError(f"{entry}: quantised activation {tuple(xq.shape)} does not match K = {qw.K}")
+    if out is None:
+        out = torch.empty((M, N), dtype=out_dtype, device=xq.device)
+    if out.dtype not in (torch.bfloat16, torch.float32) or out.stride(-1) != 1 or out.shape != (M, N):
+        raise ValueError(f"{entry}: out must be a bf16 / fp32 [M, N] tensor with contiguous rows")
+    if residual is not None and (residual.shape != out.shape or residual.stride(-1) != 1):
+        raise ValueError(f"{entry}: residual must match the output shape")
+    check(getattr(_lib.load(), entry)(ptr(xq), ptr(qw.w.wq), ptr(sa), ptr(qw.w.sw), ptr(out), M, N, K, out.stride(0),
+                                      ptr(bias), ptr(residual), residual.stride(0) if residual is not None else 0,
+                                      int(out.dtype == torch.float32), stream()), entry)
+    return out
+
+
+def gemv_fp8(qa, qw, bias=None, residual=None, out=None, out_dtype=torch.bfloat16) -> torch.Tensor:
+    """y[M, N] for M <= 8 rows (decode) from qa = fp8_quantize_act(x) and an Fp8Projection: wgmma with W as A."""
+    return _fp8_matmul("cb_gemv_fp8", qa, qw, bias, residual, out, out_dtype)
+
+
+def gemm_fp8(qa, qw, bias=None, residual=None, out=None, out_dtype=torch.bfloat16) -> torch.Tensor:
+    """The same product on the FP8 tensor-core GEMM, any M (prefill, batches above 8 rows)."""
+    return _fp8_matmul("cb_gemm_fp8", qa, qw, bias, residual, out, out_dtype)
+
+
+def fp8_linear(x, qw, residual=None, out=None, out_dtype=torch.bfloat16) -> torch.Tensor:
+    """y = x @ W^T (+ residual) on an FP8 projection (quant_fp8.Fp8Projection): the activation is quantised per row,
+    then M <= 8 rows run the GEMV and larger M the GEMM."""
+    qa = fp8_quantize_act(x)
+    if x.shape[0] <= 8:
+        return gemv_fp8(qa, qw, residual=residual, out=out, out_dtype=out_dtype)
+    return gemm_fp8(qa, qw, residual=residual, out=out, out_dtype=out_dtype)
+
+
+def fp8_mlp_gate_up(h2d, qw):
+    """`mlp_gate_up` on the stacked FP8 gate|up projection: (gu [M, 2F], act = silu(gate) * up)."""
+    gu = fp8_linear(h2d, qw)
+    I = qw.N // 2
+    return gu, swiglu_fwd(gu[:, :I], gu[:, I:])

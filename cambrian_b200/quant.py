@@ -110,18 +110,21 @@ def quantize(w: torch.Tensor, workspace: torch.Tensor | None = None) -> NF4Weigh
 
 
 def quantized_format(model) -> str | None:
-    """"4-bit (NF4)" or "8-bit (LLM.int8)" when a decoder layer of `model` carries quantised weights
-    (quantize_decoder_nf4_ / quant_int8.quantize_decoder_int8_), else None: the wording of every refusal."""
+    """"4-bit (NF4)", "8-bit (LLM.int8)" or "8-bit (FP8)" when a decoder layer of `model` carries quantised weights
+    (quantize_decoder_nf4_ / quant_int8.quantize_decoder_int8_ / quant_fp8.quantize_decoder_fp8_), else None: the
+    wording of every refusal."""
     for m in model.modules():
         if getattr(m, "_nf4", None) is not None:
             return "4-bit (NF4)"
         if getattr(m, "_int8", None) is not None:
             return "8-bit (LLM.int8)"
+        if getattr(m, "_fp8", None) is not None:
+            return "8-bit (FP8)"
     return None
 
 
 def is_quantized(model) -> bool:
-    """True when any decoder layer of `model` carries NF4 or int8 weights."""
+    """True when any decoder layer of `model` carries NF4, int8 or FP8 weights."""
     return quantized_format(model) is not None
 
 

@@ -302,6 +302,28 @@ int cb_gemv_int8(const void* xq, const void* cb, const float* sca, const float* 
 int cb_gemm_int8(const void* xq, const void* cb, const float* sca, const float* scb, const void* x, int64_t ldx,
                  const int32_t* outlier_idx, const int32_t* n_outlier, void* y, int M, int N, int K, int64_t ldy,
                  const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream);
+/* FP8 E4M3 decoder weights for inference (`load_fp8`).  The reference has no FP8 path: these replace the same seven
+ * decoder projections as the two entries above (`F.linear` in the LlamaDecoderLayer that model/builder.py:29-175 builds),
+ * with the format and the exact order of the epilogue defined in cambrian_b200/quant_fp8.py.  Per-row scales on both
+ * sides, K % 16 == 0; the same rule quantises a weight row at load and an activation row per call:
+ *   s = amax / 448, r = min(448 / amax, FLT_MAX), q[k] = e4m3_rn_satfinite(v[k] * r)   (every operation fp32-rounded);
+ *   output: y = acc * (sa[m] * sw[n]) (+ bias[n]) (+ residual[m,n]), acc = sum_k xq[m,k] * wq[n,k] in fp32, every
+ *   128-deep k-block summed on the tensor cores on its own and added in fp32 registers.
+ *
+ * cb_fp8_quantize_weight: one bf16 W [N, K] (row stride ldw) -> wq e4m3 [N, K] (row stride K), sw fp32 [N];
+ * deterministic, no host sync. */
+int cb_fp8_quantize_weight(const void* w, int N, int K, int64_t ldw, void* wq, float* sw, void* stream);
+/* x [M, K] bf16 (row stride ldx) -> xq e4m3 [M, K], sa fp32 [M]: one pass per row, no atomics, no host synchronisation
+ * (graph-capturable). */
+int cb_fp8_quantize_act(const void* x, int M, int K, int64_t ldx, void* xq, float* sa, void* stream);
+/* y[M,N] (bf16 or fp32, row stride ldy) from the quantised activation (xq, sa) and weight (wq, sw) — M <= 8 rows
+ * (decode): wgmma m64n8k32 with W as the A operand, K split over a thread-block cluster and reduced in rank order; any
+ * M: tensor-core GEMM (wgmma m64n128k32 .f32.e4m3.e4m3).  Both deterministic run to run; their summation orders
+ * differ, so they agree to fp32 accumulation error, not bit for bit. */
+int cb_gemv_fp8(const void* xq, const void* wq, const float* sa, const float* sw, void* y, int M, int N, int K,
+                int64_t ldy, const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream);
+int cb_gemm_fp8(const void* xq, const void* wq, const float* sa, const float* sw, void* y, int M, int N, int K,
+                int64_t ldy, const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream);
 
 #ifdef __cplusplus
 }
