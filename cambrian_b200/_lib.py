@@ -87,6 +87,9 @@ SIGNATURES = {
     "cb_fp8_quantize_act": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp]),
     "cb_gemv_fp8": (_i, [_vp] * 5 + [_i, _i, _i, _i64, _vp, _vp, _i64, _i, _vp]),
     "cb_gemm_fp8": (_i, [_vp] * 5 + [_i, _i, _i, _i64, _vp, _vp, _i64, _i, _vp]),
+    "cb_kv_fp8_append": (_i, [_vp, _vp, _i64] + [_vp] * 4 + [_i] * 5 + [_i64, _vp, _vp]),
+    "cb_attn_decode_fp8_workspace_floats": (_i64, [_i] * 5),
+    "cb_attn_decode_fp8": (_i, [_vp, _i64] + [_vp] * 5 + [_i64, _vp, _vp, _i64] + [_i] * 6 + [_i64, _vp, _f, _vp]),
 }
 
 _lib = None

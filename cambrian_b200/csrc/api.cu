@@ -125,6 +125,12 @@ int gemv_fp8_launch(const void*, const void*, const float*, const float*, void*,
                     const void*, long long, int, cudaStream_t);
 int gemm_fp8_launch(const void*, const void*, const float*, const float*, void*, int, int, int, long long, const void*,
                     const void*, long long, int, cudaStream_t);
+int kv_fp8_append_launch(const void*, const void*, long long, void*, void*, float*, float*, int, int, int, int, int, long long,
+                         const long long*, cudaStream_t);
+long long attn_decode_fp8_workspace_floats(int, int, int, int, int);
+int attn_decode_fp8_launch(const void*, long long, const void*, const void*, const float*, const float*, const void*, long long,
+                           void*, float*, long long, int, int, int, int, int, int, long long, const long long*, float,
+                           cudaStream_t);
 
 }  // namespace cb
 
@@ -407,6 +413,21 @@ int cb_gemv_fp8(const void* xq, const void* wq, const float* sa, const float* sw
 int cb_gemm_fp8(const void* xq, const void* wq, const float* sa, const float* sw, void* y, int M, int N, int K,
                 int64_t ldy, const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream) {
   return cb::gemm_fp8_launch(xq, wq, sa, sw, y, M, N, K, ldy, bias, residual, ldr, out_fp32, ST(stream));
+}
+int cb_kv_fp8_append(const void* k, const void* v, int64_t ld, void* kq, void* vq, float* ks, float* vs, int B, int S,
+                     int S_max, int nkv, int hd, int64_t offset, const int64_t* offset_dev, void* stream) {
+  return cb::kv_fp8_append_launch(k, v, ld, kq, vq, ks, vs, B, S, S_max, nkv, hd, offset,
+                                  reinterpret_cast<const long long*>(offset_dev), ST(stream));
+}
+int64_t cb_attn_decode_fp8_workspace_floats(int B, int nh, int nkv, int S_max, int hd) {
+  return cb::attn_decode_fp8_workspace_floats(B, nh, nkv, S_max, hd);
+}
+int cb_attn_decode_fp8(const void* q, int64_t q_bs, const void* kq, const void* vq, const float* ks, const float* vs,
+                       const void* kmask, int64_t kmask_ld, void* o, float* workspace, int64_t workspace_floats, int B, int Sq,
+                       int nh, int nkv, int S_max, int hd, int64_t length, const int64_t* length_dev, float scale,
+                       void* stream) {
+  return cb::attn_decode_fp8_launch(q, q_bs, kq, vq, ks, vs, kmask, kmask_ld, o, workspace, workspace_floats, B, Sq, nh, nkv,
+                                    S_max, hd, length, reinterpret_cast<const long long*>(length_dev), scale, ST(stream));
 }
 
 }  // extern "C"

@@ -212,6 +212,8 @@ class CBLlamaDecoderLayer(nn.Module):
         v_new = qkv[:, (nh + nkv) * hd:].view(B, S, nkv, hd)
         if cache is None:
             attn = ops.attn_fwd(q, k_new, v_new, causal=True, kmask=rt["kmask"])
+        elif cache.fp8 is not None:
+            attn = self._attn_fp8_cache(q, k_new, v_new, cache, rt["kmask"])
         elif cache.slot is not None:
             # static-shape decode step (CUDA-graph replay): the write slot is a DEVICE index, attention runs over the whole
             # cache buffer and the validity mask (updated on the device) hides the slots not written yet
@@ -238,18 +240,48 @@ class CBLlamaDecoderLayer(nn.Module):
         _, act = ops.mlp_gate_up(h2, gu_w)
         return ops.gemm(act, m.down_proj.weight, residual=x1).view(B, S, H)
 
+    def _attn_fp8_cache(self, q, k_new, v_new, cache, kmask):
+        """Attention with the FP8 cache (kv_fp8.py): the prompt attends over its own bf16 K / V and is then appended; a
+        decode step appends its row, then attends over the quantised cache up to and including it."""
+        kq, vq, ks, vs = cache.fp8.layer(self.layer_idx)
+        S = q.shape[1]
+        if cache.slot is None and cache.length == 0:
+            attn = ops.attn_fwd(q, k_new, v_new, causal=True, kmask=kmask)
+            ops.kv_fp8_append(k_new, v_new, kq, vq, ks, vs, offset=0)
+            return attn
+        if S != 1:
+            raise NotImplementedError("an FP8 KV cache takes a prompt into an empty cache or one token per decode step, "
+                                      f"not {S} tokens after {cache.length} cached positions")
+        if cache.slot is not None:       # graph-replayed step: write slot and valid length come from the device slot
+            ops.kv_fp8_append(k_new, v_new, kq, vq, ks, vs, offset=0, offset_dev=cache.slot)
+            return ops.attn_decode_fp8(q, kq, vq, ks, vs, cache.fp8.ws, length=1, length_dev=cache.slot, kmask=kmask)
+        t0 = cache.length
+        ops.kv_fp8_append(k_new, v_new, kq, vq, ks, vs, offset=t0)
+        return ops.attn_decode_fp8(q, kq, vq, ks, vs, cache.fp8.ws, length=t0 + 1, kmask=kmask)
+
 
 class KVCache:
-    """Per-layer [B, S_max, n_kv, head_dim] bf16 buffers (the layout the attention kernel's TMA maps address)."""
+    """Per-layer [B, S_max, n_kv, head_dim] bf16 buffers (the layout the attention kernel's TMA maps address), or with
+    dtype="fp8" the E4M3 rows and fp32 scales of kv_fp8.py plus the decode workspace (`fp8`)."""
 
-    def __init__(self, config, batch, max_len, device):
+    def __init__(self, config, batch, max_len, device, dtype="bf16"):
+        from ...kv_fp8 import CACHE_DTYPES, Fp8KVLayers
+        if dtype not in CACHE_DTYPES:
+            raise ValueError(f"KVCache dtype {dtype!r} is not supported: use one of {CACHE_DTYPES}")
         nkv = config.num_key_value_heads
         hd = getattr(config, "head_dim", None) or config.hidden_size // config.num_attention_heads
         L = config.num_hidden_layers
-        # zero-initialised: the static-shape decode step attends over the WHOLE buffer with not-yet-written slots masked
-        # out — their probabilities are exactly 0, but 0 x (uninitialised NaN / Inf bit patterns in V) would still be NaN
-        self.k = [torch.zeros((batch, max_len, nkv, hd), dtype=torch.bfloat16, device=device) for _ in range(L)]
-        self.v = [torch.zeros((batch, max_len, nkv, hd), dtype=torch.bfloat16, device=device) for _ in range(L)]
+        self.dtype = dtype
+        self.fp8 = None
+        if dtype == "fp8":
+            self.k = self.v = None
+            self.fp8 = Fp8KVLayers(L, batch, max_len, config.num_attention_heads, nkv, hd, device)
+        else:
+            # zero-initialised: the static-shape decode step attends over the WHOLE buffer with not-yet-written slots
+            # masked out — their probabilities are exactly 0, but 0 x (uninitialised NaN / Inf bit patterns in V) would
+            # still be NaN
+            self.k = [torch.zeros((batch, max_len, nkv, hd), dtype=torch.bfloat16, device=device) for _ in range(L)]
+            self.v = [torch.zeros((batch, max_len, nkv, hd), dtype=torch.bfloat16, device=device) for _ in range(L)]
         self.length = 0
         self.max_len = max_len
         self.kmask = None  # [B, max_len] bool, key validity over the whole cache
@@ -257,6 +289,12 @@ class KVCache:
 
     def get_seq_length(self):
         return self.length
+
+    def nbytes(self) -> int:
+        """Device bytes the cache holds (for fp8: rows, scales and the decode workspace)."""
+        if self.fp8 is not None:
+            return self.fp8.nbytes()
+        return sum(t.numel() * t.element_size() for t in self.k + self.v)
 
 
 class CambrianPreTrainedModel(PreTrainedModel):
@@ -519,10 +557,18 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
         `pad_token_id`, `max_new_tokens` / `max_length`, `stopping_criteria`, `streamer`, `attention_mask`,
         `position_ids`, `generation_config`, `generator`.  Any other keyword is rejected unless it carries its neutral
         value (num_beams=1, use_cache=True, ...).  Returns the newly generated ids [B, T], as HF does when generation
-        starts from `inputs_embeds`."""
+        starts from `inputs_embeds`.
+
+        `kv_cache_dtype` ("bf16" or "fp8", default `config.kv_cache_dtype` or "bf16") selects the decode KV cache:
+        "fp8" keeps it in E4M3 with per-row scales (cambrian_b200/kv_fp8.py), about half the bytes of bf16."""
         from ...generation import GenerationArgs, next_tokens, should_stop
+        from ...kv_fp8 import resolve_cache_dtype
         if "inputs_embeds" in kwargs:
             raise NotImplementedError("`inputs_embeds` is not supported")                       # :447-448
+        kv_dtype = resolve_cache_dtype(self.config, kwargs.pop("kv_cache_dtype", None))
+        z3 = getattr(self.get_model(), "_zero3", None)
+        if z3 is not None and kv_dtype == "fp8":
+            raise NotImplementedError("kv_cache_dtype='fp8' is not supported with Zero3Inference")
         sync = getattr(self, "_cb_param_sync", None)
         if sync is not None:
             sync()      # a TrainEngine with deferred parameter sync: inference kernels read parameters directly
@@ -542,7 +588,7 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
         args = GenerationArgs.from_kwargs(self, S0, kwargs)
         max_new = args.max_new_tokens
         dev = inputs.device
-        cache = KVCache(self.config, B, S0 + max_new, dev)
+        cache = KVCache(self.config, B, S0 + max_new, dev, dtype=kv_dtype)
         cache.kmask = torch.ones((B, S0 + max_new), dtype=torch.bool, device=dev)
         if attention_mask is not None:
             cache.kmask[:, :S0] = attention_mask.bool()
@@ -557,7 +603,6 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
         h_last = out.last_hidden_state[torch.arange(B, device=dev), last_idx].contiguous()
         next_pos = (position_ids.max(1).values + 1) if position_ids is not None else torch.full((B,), S0, device=dev)
         done = torch.zeros(B, dtype=torch.bool, device=dev)
-        z3 = getattr(self.get_model(), "_zero3", None)
         check_stop = bool(args.eos_token_ids or args.stopping_criteria)
         if args.streamer is not None:
             args.streamer.put(torch.empty((B, 0), dtype=torch.long))     # HF streams the (here: empty) prompt ids first

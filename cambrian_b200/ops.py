@@ -940,3 +940,68 @@ def fp8_mlp_gate_up(h2d, qw):
     gu = fp8_linear(h2d, qw)
     I = qw.N // 2
     return gu, swiglu_fwd(gu[:, :I], gu[:, I:])
+
+
+# ------------------------------------------------------------------------------------------------
+# FP8 E4M3 decode KV cache (kv_cache_dtype="fp8"; the format and the decode arithmetic live in kv_fp8.py)
+# ------------------------------------------------------------------------------------------------
+def kv_fp8_append(k, v, kq, vq, ks, vs, offset: int = 0, offset_dev=None):
+    """Quantise the new rows k, v [B, S, nkv, hd] (views of the packed post-RoPE qkv rows, read in place) into one
+    layer's FP8 cache kq, vq [B, S_max, nkv, hd] float8_e4m3fn, ks, vs [B, S_max, nkv] fp32 at positions offset + s
+    (+ offset_dev[0], a device int64, for the graph-replayed step)."""
+    _require_cuda_bf16(k, v)
+    B, S, nkv, hd = k.shape
+    # the row stride: a size-1 dimension's stride says nothing, so one token per sequence takes it from the batch stride
+    ld = k.stride(1) if S > 1 else (k.stride(0) if B > 1 else nkv * hd)
+    if (v.shape != k.shape or v.stride() != k.stride() or k.stride(3) != 1 or (nkv > 1 and k.stride(2) != hd)
+            or (B > 1 and k.stride(0) != S * ld)):
+        raise ValueError(f"kv_fp8_append: k, v must be [B, S, nkv, hd] rows at one common stride, got {k.stride()}")
+    S_max = kq.shape[1]
+    if (kq.shape != (B, S_max, nkv, hd) or vq.shape != kq.shape or kq.dtype != torch.float8_e4m3fn
+            or vq.dtype != kq.dtype or ks.shape != (B, S_max, nkv) or vs.shape != ks.shape or ks.dtype != torch.float32
+            or vs.dtype != torch.float32 or not all(t.is_contiguous() for t in (kq, vq, ks, vs))):
+        raise ValueError("kv_fp8_append: cache buffers must be contiguous kq, vq float8_e4m3fn [B, S_max, nkv, hd] and "
+                         "ks, vs fp32 [B, S_max, nkv]")
+    if offset_dev is not None and (offset_dev.dtype != torch.int64 or offset_dev.numel() != 1):
+        raise ValueError("kv_fp8_append: offset_dev must be one device int64")
+    check(_lib.load().cb_kv_fp8_append(ptr(k), ptr(v), ld, ptr(kq), ptr(vq), ptr(ks), ptr(vs), B, S, S_max, nkv,
+                                       hd, int(offset), ptr(offset_dev), stream()), "cb_kv_fp8_append")
+
+
+def attn_decode_fp8_workspace(B: int, nh: int, nkv: int, S_max: int, hd: int, device) -> torch.Tensor:
+    """The fp32 workspace `attn_decode_fp8` needs for this shape on `device` (at least one element)."""
+    with torch.cuda.device(device):
+        n = _lib.load().cb_attn_decode_fp8_workspace_floats(B, nh, nkv, S_max, hd)
+    return torch.empty(max(int(n), 1), dtype=torch.float32, device=device)
+
+
+def attn_decode_fp8(q, kq, vq, ks, vs, workspace, *, length: int, length_dev=None, kmask=None,
+                    scale: float | None = None):
+    """Decode attention over one layer's FP8 cache: q [B, 1, nh, hd] (a view of the packed qkv row) -> o [B, 1, nh, hd]
+    bf16.  Valid keys: positions below length (+ length_dev[0]), with kmask [B, >= those positions] set."""
+    _require_cuda_bf16(q)
+    B, Sq, nh, hd = q.shape
+    S_max, nkv = kq.shape[1], kq.shape[2]
+    if scale is None:
+        scale = hd ** -0.5
+    qb, _ = _bshd_strides(q, hd)
+    if (kq.dtype != torch.float8_e4m3fn or vq.dtype != kq.dtype or ks.dtype != torch.float32 or vs.dtype != torch.float32
+            or kq.shape != (B, S_max, nkv, hd) or vq.shape != kq.shape or ks.shape != (B, S_max, nkv)
+            or vs.shape != ks.shape or not all(t.is_contiguous() for t in (kq, vq, ks, vs))):
+        raise ValueError("attn_decode_fp8: cache buffers must be contiguous kq, vq float8_e4m3fn [B, S_max, nkv, hd] and "
+                         "ks, vs fp32 [B, S_max, nkv]")
+    if workspace.dtype != torch.float32:
+        raise ValueError("attn_decode_fp8: the workspace must be fp32")
+    if length_dev is not None and (length_dev.dtype != torch.int64 or length_dev.numel() != 1):
+        raise ValueError("attn_decode_fp8: length_dev must be one device int64")
+    km, km_ld = None, 0
+    if kmask is not None:
+        if kmask.dim() != 2 or kmask.shape[0] != B or kmask.stride(1) != 1:
+            raise ValueError("attn_decode_fp8: kmask must be [B, positions] with contiguous rows")
+        km = kmask.view(torch.uint8) if kmask.dtype == torch.bool else kmask.to(torch.uint8)
+        km_ld = km.stride(0) if B > 1 else km.shape[1]
+    o = torch.empty((B, Sq, nh, hd), dtype=torch.bfloat16, device=q.device)
+    check(_lib.load().cb_attn_decode_fp8(ptr(q), qb, ptr(kq), ptr(vq), ptr(ks), ptr(vs), ptr(km), km_ld, ptr(o),
+                                         ptr(workspace), workspace.numel(), B, Sq, nh, nkv, S_max, hd, int(length),
+                                         ptr(length_dev), float(scale), stream()), "cb_attn_decode_fp8")
+    return o

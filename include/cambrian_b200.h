@@ -324,6 +324,30 @@ int cb_gemv_fp8(const void* xq, const void* wq, const float* sa, const float* sw
                 int64_t ldy, const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream);
 int cb_gemm_fp8(const void* xq, const void* wq, const float* sa, const float* sw, void* y, int M, int N, int K,
                 int64_t ldy, const void* bias, const void* residual, int64_t ldr, int out_fp32, void* stream);
+/* FP8 E4M3 decode KV cache (`generate(..., kv_cache_dtype="fp8")`; the format and the decode arithmetic are defined in
+ * cambrian_b200/kv_fp8.py).  The reference keeps HF's bf16 DynamicCache behind LlamaSdpaAttention (the decode steps of
+ * cambrian_llama.py:437-483 through GenerationMixin.generate); these replace its cache update and the decode-step SDPA.
+ * Per layer: kq, vq e4m3 [B, S_max, nkv, hd] and ks, vs fp32 [B, S_max, nkv]; every (sequence, position, kv head) row of
+ * K or V is quantised by the cb_fp8_quantize_act rule (s = amax / 448, q = e4m3_rn_satfinite(x * r)).  hd 64 or 128.
+ *
+ * cb_kv_fp8_append: the new rows k, v (element (b, s, h, d) at base + (b * S + s) * ld + h * hd + d: the K and V heads of
+ * the packed post-RoPE qkv rows, read in place) go to positions offset + s, plus *offset_dev when offset_dev is not NULL
+ * (the device write slot of the graph-replayed decode step; a position past S_max is then skipped). */
+int cb_kv_fp8_append(const void* k, const void* v, int64_t ld, void* kq, void* vq, float* ks, float* vs, int B, int S,
+                     int S_max, int nkv, int hd, int64_t offset, const int64_t* offset_dev, void* stream);
+/* fp32 workspace cb_attn_decode_fp8 needs for this shape on the current device (0: one split, no workspace) */
+int64_t cb_attn_decode_fp8_workspace_floats(int B, int nh, int nkv, int S_max, int hd);
+/* Decode attention over the FP8 cache (flash-decoding), one query per sequence (Sq == 1): q element (b, h, d) at
+ * q + b * q_bs + h * hd + d (a view of the packed qkv row), o [B, nh, hd] bf16 contiguous.  Valid keys: positions below
+ * length (+ *length_dev when not NULL), clipped to S_max, and with kmask [B, kmask_ld] (1 byte, 1 = attend; may be NULL)
+ * set.  One CTA per (key split, kv head, sequence) serves the nh / nkv (1..8) query heads of that kv head, so each cache
+ * byte is read once per call, and only below the valid length.  The split count is a function of (B, nkv, S_max, SM
+ * count); with more than one split the partial results are merged in split order through `workspace` (no atomics):
+ * bit-identical from run to run. */
+int cb_attn_decode_fp8(const void* q, int64_t q_bs, const void* kq, const void* vq, const float* ks, const float* vs,
+                       const void* kmask, int64_t kmask_ld, void* o, float* workspace, int64_t workspace_floats, int B, int Sq,
+                       int nh, int nkv, int S_max, int hd, int64_t length, const int64_t* length_dev, float scale,
+                       void* stream);
 
 #ifdef __cplusplus
 }

@@ -2,10 +2,13 @@
 prefill, against the weight-streaming floor (bf16 weights / measured HBM bandwidth).
 
     python tools/decode_bench.py [--batch 1] [--prompt 1024] [--new 64] [--config 8b-ddp | yi34b] [--load-4bit | --load-8bit | --load-fp8]
+                                 [--kv-fp8]
 
 --load-4bit quantises the decoder projections to NF4 (cambrian_b200/quant.py), --load-8bit to LLM.int8
 (cambrian_b200/quant_int8.py), --load-fp8 to FP8 E4M3 (cambrian_b200/quant_fp8.py), layer by layer after building the model on the CPU, so configurations whose bf16 decoder
 does not fit one GPU (--config yi34b: Cambrian-34B-shaped, 60 layers) run.  8-bit takes precedence, as in the loader.
+--kv-fp8 runs every batch twice in the same session, with the bf16 KV cache and then with the FP8 one
+(generate(kv_cache_dtype="fp8"), cambrian_b200/kv_fp8.py), and adds the cache's KVCache.nbytes() to each line.
 """
 import argparse
 import json
@@ -32,6 +35,7 @@ def main():
     ap.add_argument("--load-8bit", action="store_true", help="LLM.int8 decoder projections (quant_int8)")
     ap.add_argument("--load-fp8", action="store_true", help="FP8 E4M3 decoder projections (quant_fp8)")
     ap.add_argument("--layers", type=int, default=60, help="decoder layers of --config yi34b")
+    ap.add_argument("--kv-fp8", action="store_true", help="each batch with the bf16 and then the FP8 KV cache")
     args = ap.parse_args()
     from cambrian_b200 import quant, quant_fp8, quant_int8
     from cambrian_b200.model.language_model.cambrian_llama import CambrianLlamaForCausalLM
@@ -72,16 +76,24 @@ def main():
     torch.cuda.reset_peak_memory_stats()
     model._bench_qstats = qstats
     for B in [int(b) for b in str(args.batch).split(",")]:
-        one_batch(args, model, cfg, dev, B)
+        for kv in (("bf16", "fp8") if args.kv_fp8 else (None,)):
+            one_batch(args, model, cfg, dev, B, kv)
 
 
-def one_batch(args, model, cfg, dev, B):
+def one_batch(args, model, cfg, dev, B, kv=None):
     from cambrian_b200 import _lib
     C = bench.CONFIGS["8b-ddp"] if args.config == "yi34b" else bench.CONFIGS[args.config]
     ids = torch.randint(3, cfg.vocab_size, (B, args.prompt - 599), device=dev)
     ids[:, cfg.image_position] = -200
     images = [torch.randn(B, 3, r, r, device=dev).bfloat16() for r in C["res"]]
     kw = dict(images=images, image_sizes=[(336, 336)] * B, do_sample=False)
+    kv_bytes = None
+    if kv is not None:
+        from cambrian_b200.model.language_model.cambrian_llama import KVCache
+        kw["kv_cache_dtype"] = kv
+        kv_bytes = KVCache(cfg, B, args.prompt + args.new + 1, dev, dtype=kv).nbytes()   # the cache generate() builds
+        torch.cuda.empty_cache()
+        torch.cuda.reset_peak_memory_stats()
 
     def run(n):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -120,7 +132,7 @@ def one_batch(args, model, cfg, dev, B):
         top = [dict(kernel=k, ms_per_token=round(v[0] / 1e3 / args.new, 4), launches_per_token=round(v[1] / args.new, 1))
                for k, v in sorted(agg.items(), key=lambda kv: -kv[1][0])[:14]]
     print(json.dumps(dict(metric="decode_ms_per_token", value=ms_tok, unit="ms", config=args.config, load_4bit=args.load_4bit and not args.load_8bit,
-                          load_8bit=args.load_8bit, load_fp8=args.load_fp8,
+                          load_8bit=args.load_8bit, load_fp8=args.load_fp8, kv_cache_dtype=kv, kv_cache_bytes=kv_bytes,
                           batch=B, prompt=args.prompt, new_tokens=args.new, prefill_ms=t1, tokens_per_s=B * 1000.0 / ms_tok,
                           launches_per_token=(ln - l1) / args.new, decode_graph=not args.no_graph, weight_bytes=weight_bytes,
                           decoder_nf4_bytes=qstats.get("nf4_bytes") if qstats else None,
