@@ -90,6 +90,10 @@ SIGNATURES = {
     "cb_kv_fp8_append": (_i, [_vp, _vp, _i64] + [_vp] * 4 + [_i] * 5 + [_i64, _vp, _vp]),
     "cb_attn_decode_fp8_workspace_floats": (_i64, [_i] * 5),
     "cb_attn_decode_fp8": (_i, [_vp, _i64] + [_vp] * 5 + [_i64, _vp, _vp, _i64] + [_i] * 6 + [_i64, _vp, _f, _vp]),
+    "cb_fp8_quantize_weight_t_workspace_floats": (_i64, [_i, _i]),
+    "cb_fp8_quantize_weight_t": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp, _i64, _vp]),
+    "cb_rmsnorm_fwd_fp8": (_i, [_vp] * 5 + [_i64, _i, _f, _i, _vp]),
+    "cb_swiglu_bwd_fp8": (_i, [_vp] * 7 + [_i64, _i, _i64, _i64, _i64, _vp]),
 }
 
 _lib = None

@@ -13,7 +13,7 @@ from __future__ import annotations
 
 import torch
 
-from . import ops
+from . import ops, train_fp8
 
 
 def _ranged(tag):
@@ -611,7 +611,8 @@ class DecoderLayerFn(torch.autograd.Function):
     """x [B,S,H] -> x'.  Parameters: input_ln, qkv_w (fused [ (nh+2nkv)*hd, H ]), o_w, post_ln, gu_w (fused [2I, H]), down_w.
 
     meta = dict(nh, nkv, hd, eps, hf_cast, cos, sin, pos (int64 [B*S]), kmask (bool [B,S] or None), params (6 Parameters),
-                recompute (bool: keep only x and redo the forward in backward — per-layer activation checkpointing))
+                recompute (bool: keep only x and redo the forward in backward — per-layer activation checkpointing),
+                fp8 (bool, optional: the four projection GEMMs and their input-gradient GEMMs in E4M3, train_fp8.py))
     """
 
     @staticmethod
@@ -619,22 +620,39 @@ class DecoderLayerFn(torch.autograd.Function):
         B, S, H = x.shape
         nh, nkv, hd = meta["nh"], meta["nkv"], meta["hd"]
         rows = B * S
+        fp8 = meta.get("fp8", False)
         x2 = x.reshape(rows, H)
-        h, rstd1 = ops.rmsnorm_fwd(x2, ln1, meta["eps"], meta["hf_cast"], save_stats=True)
-        qkv = ops.gemm(h, qkv_w)
+        if fp8:  # train_fp8.py: each weight quantised row-wise here, per call; activations per token
+            hq, rstd1 = ops.rmsnorm_fwd_fp8(x2, ln1, meta["eps"], meta["hf_cast"])
+            qkv = ops.gemm_fp8(hq, train_fp8.weight_rows(qkv_w))
+            del hq
+        else:
+            h, rstd1 = ops.rmsnorm_fwd(x2, ln1, meta["eps"], meta["hf_cast"], save_stats=True)
+            qkv = ops.gemm(h, qkv_w)
         ops.rope_(qkv, meta["pos"], meta["cos"], meta["sin"], nh + nkv, hd)
         q = qkv[:, : nh * hd].view(B, S, nh, hd)
         k = qkv[:, nh * hd:(nh + nkv) * hd].view(B, S, nkv, hd)
         v = qkv[:, (nh + nkv) * hd:].view(B, S, nkv, hd)
         attn, lse = ops.attn_fwd(q, k, v, causal=True, kmask=meta["kmask"], need_lse=True)
         attn2 = attn.view(rows, nh * hd)
-        x1 = ops.gemm(attn2, o_w, residual=x2)
-        h2, rstd2 = ops.rmsnorm_fwd(x1, ln2, meta["eps"], meta["hf_cast"], save_stats=True)
-        gu, act = ops.mlp_gate_up(h2, gu_w)
+        if fp8:
+            x1 = ops.gemm_fp8(ops.fp8_quantize_act(attn2), train_fp8.weight_rows(o_w), residual=x2)
+            h2q, rstd2 = ops.rmsnorm_fwd_fp8(x1, ln2, meta["eps"], meta["hf_cast"])
+            gu = ops.gemm_fp8(h2q, train_fp8.weight_rows(gu_w))
+            del h2q
+            I = gu_w.shape[0] // 2
+            act = ops.swiglu_fwd(gu[:, :I], gu[:, I:])
+        else:
+            x1 = ops.gemm(attn2, o_w, residual=x2)
+            h2, rstd2 = ops.rmsnorm_fwd(x1, ln2, meta["eps"], meta["hf_cast"], save_stats=True)
+            gu, act = ops.mlp_gate_up(h2, gu_w)
         saved = (rstd1, qkv, attn, lse, x1, rstd2, gu, act) if keep else None
         if not need_out:  # the backward's recompute needs only the saved activations, not the layer's output
             return None, saved
-        out = ops.gemm(act, down_w, residual=x1)
+        if fp8:
+            out = ops.gemm_fp8(ops.fp8_quantize_act(act), train_fp8.weight_rows(down_w), residual=x1)
+        else:
+            out = ops.gemm(act, down_w, residual=x1)
         return out.view(B, S, H), saved
 
     @staticmethod
@@ -672,22 +690,38 @@ class DecoderLayerFn(torch.autograd.Function):
         I = gu_w.shape[0] // 2
         x2 = x.reshape(rows, H)
         dx2 = dout.reshape(rows, H).contiguous()
+        # dgrad: dX = dY W, either bf16 (W as the MN-major operand) or E4M3 on W^T quantised here, per call (train_fp8.py)
+        fp8 = meta.get("fp8", False)
+        if fp8:
+            _await(*meta["params"])
+
+        def dgrad(dy, w):
+            if fp8:
+                return ops.gemm_fp8(ops.fp8_quantize_act(dy), train_fp8.weight_t(w))
+            return ops.gemm(dy, w, b_mn=True)
+
         # ---- MLP
         h2 = ops.rmsnorm_fwd(x1, ln2, meta["eps"], meta["hf_cast"])       # cheap recompute (bandwidth only)
-        dact = ops.gemm(dx2, down_w, b_mn=True)
+        dact = dgrad(dx2, down_w)
         g_down = wgrad(p_down, dx2, act)
         del act
         dgu = torch.empty_like(gu)
-        ops.swiglu_bwd(dact, gu[:, :I], gu[:, I:], dgu[:, :I], dgu[:, I:])
-        del dact
-        dh2 = ops.gemm(dgu, gu_w, b_mn=True)
+        if fp8:  # the bf16 dgu feeds the gate|up wgrad, its E4M3 rows the gate|up dgrad
+            dguq = ops.swiglu_bwd_fp8(dact, gu[:, :I], gu[:, I:], dgu[:, :I], dgu[:, I:])
+            del dact
+            dh2 = ops.gemm_fp8(dguq, train_fp8.weight_t(gu_w))
+            del dguq
+        else:
+            ops.swiglu_bwd(dact, gu[:, :I], gu[:, I:], dgu[:, :I], dgu[:, I:])
+            del dact
+            dh2 = ops.gemm(dgu, gu_w, b_mn=True)
         g_gu = wgrad(p_gu, dgu, h2)
         del dgu, h2
         dx1, dg2 = ops.rmsnorm_bwd(dh2, x1, ln2, rstd2, dres=dx2)
         g_ln2 = vgrad(p_ln2, dg2)
         # ---- attention
         attn2 = attn.view(rows, nh * hd)
-        dattn = ops.gemm(dx1, o_w, b_mn=True)
+        dattn = dgrad(dx1, o_w)
         g_o = wgrad(p_o, dx1, attn2)
         dqkv = torch.empty_like(qkv)
         q = qkv[:, : nh * hd].view(B, S, nh, hd)
@@ -698,7 +732,7 @@ class DecoderLayerFn(torch.autograd.Function):
                      dv=dqkv[:, (nh + nkv) * hd:].view(B, S, nkv, hd))
         ops.rope_(dqkv, meta["pos"], meta["cos"], meta["sin"], nh + nkv, hd, inverse=True)
         h = ops.rmsnorm_fwd(x2, ln1, meta["eps"], meta["hf_cast"])
-        dh = ops.gemm(dqkv, qkv_w, b_mn=True)
+        dh = dgrad(dqkv, qkv_w)
         g_qkv = wgrad(p_qkv, dqkv, h)
         del dqkv, h
         dx, dg1 = ops.rmsnorm_bwd(dh, x2, ln1, rstd1, dres=dx1)

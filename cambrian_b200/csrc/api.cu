@@ -131,6 +131,11 @@ long long attn_decode_fp8_workspace_floats(int, int, int, int, int);
 int attn_decode_fp8_launch(const void*, long long, const void*, const void*, const float*, const float*, const void*, long long,
                            void*, float*, long long, int, int, int, int, int, int, long long, const long long*, float,
                            cudaStream_t);
+long long fp8_quantize_weight_t_workspace_floats(int, int);
+int fp8_quantize_weight_t_launch(const void*, int, int, long long, void*, float*, float*, long long, cudaStream_t);
+int rmsnorm_fwd_fp8(const void*, const void*, void*, float*, float*, long long, int, float, int, cudaStream_t);
+int swiglu_bwd_fp8_launch(const void*, const void*, const void*, void*, void*, void*, float*, long long, int, long long,
+                          long long, long long, cudaStream_t);
 
 }  // namespace cb
 
@@ -428,6 +433,21 @@ int cb_attn_decode_fp8(const void* q, int64_t q_bs, const void* kq, const void* 
                        void* stream) {
   return cb::attn_decode_fp8_launch(q, q_bs, kq, vq, ks, vs, kmask, kmask_ld, o, workspace, workspace_floats, B, Sq, nh, nkv,
                                     S_max, hd, length, reinterpret_cast<const long long*>(length_dev), scale, ST(stream));
+}
+int64_t cb_fp8_quantize_weight_t_workspace_floats(int N, int K) {
+  return cb::fp8_quantize_weight_t_workspace_floats(N, K);
+}
+int cb_fp8_quantize_weight_t(const void* w, int N, int K, int64_t ldw, void* wtq, float* st, float* workspace,
+                             int64_t workspace_floats, void* stream) {
+  return cb::fp8_quantize_weight_t_launch(w, N, K, ldw, wtq, st, workspace, workspace_floats, ST(stream));
+}
+int cb_rmsnorm_fwd_fp8(const void* x, const void* gamma, void* xq, float* sa, float* rstd, int64_t rows, int C, float eps,
+                       int hf_cast, void* stream) {
+  return cb::rmsnorm_fwd_fp8(x, gamma, xq, sa, rstd, rows, C, eps, hf_cast, ST(stream));
+}
+int cb_swiglu_bwd_fp8(const void* dout, const void* gate, const void* up, void* dgate, void* dup, void* dguq, float* sdgu,
+                      int64_t rows, int I, int64_t ld_in, int64_t ld_dout, int64_t ld_dgu, void* stream) {
+  return cb::swiglu_bwd_fp8_launch(dout, gate, up, dgate, dup, dguq, sdgu, rows, I, ld_in, ld_dout, ld_dgu, ST(stream));
 }
 
 }  // extern "C"

@@ -132,6 +132,17 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
   for (int i = 0; i < 4; ++i) p[i] = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
   return u;
 }
+// two fp32 -> two e4m3 (round to nearest even, |x| > 448 -> +-448); lo in the low byte (the FP8 row rule of
+// quant_fp8.py, shared by every kernel that writes e4m3)
+__device__ __forceinline__ uint32_t f8_pack2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// 8 fp32 (already scaled by r) -> 8 e4m3 bytes, element 0 in the lowest byte
+__device__ __forceinline__ uint2 f8_pack8(const float* v) {
+  return make_uint2(f8_pack2(v[0], v[1]) | f8_pack2(v[2], v[3]) << 16, f8_pack2(v[4], v[5]) | f8_pack2(v[6], v[7]) << 16);
+}
 __device__ __forceinline__ uint4 ldg_nc(const void* p) {
   uint4 r;
   asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"

@@ -3,6 +3,7 @@
 // All kernels use 16-byte vector accesses on the contiguous channel dimension (C % 8 == 0), fp32 math,
 // grid-stride loops sized in multiples of the SM count.  Reference call sites are cited per kernel.
 #include "common.cuh"
+#include <cfloat>
 #include <climits>
 
 namespace cb {
@@ -90,6 +91,16 @@ __global__ void swiglu_fwd_kernel(const bf16* __restrict__ gate, const bf16* __r
     *reinterpret_cast<uint4*>(out + r * ld_out + c) = pack8(g);
   }
 }
+// d / dgate and d / dup of out = silu(gate) * up for 8 elements (the swiglu_bwd kernels share it, so both give the
+// same bits)
+__device__ __forceinline__ void swiglu_grad8(const float* d, const float* g, const float* u, float* dg, float* du) {
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    const float s = 1.f / (1.f + __expf(-g[e]));
+    du[e] = d[e] * g[e] * s;
+    dg[e] = d[e] * u[e] * s * (1.f + g[e] * (1.f - s));
+  }
+}
 __global__ void swiglu_bwd_kernel(const bf16* __restrict__ dout, const bf16* __restrict__ gate,
                                   const bf16* __restrict__ up, bf16* __restrict__ dgate, bf16* __restrict__ dup,
                                   long long rows, int I, long long ld_in, long long ld_dout, long long ld_dgu) {
@@ -102,14 +113,54 @@ __global__ void swiglu_bwd_kernel(const bf16* __restrict__ dout, const bf16* __r
     unpack8(ldg_nc(gate + r * ld_in + c), g);
     unpack8(ldg_nc(up + r * ld_in + c), u);
     unpack8(ldg_nc(dout + r * ld_dout + c), d);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const float s = 1.f / (1.f + __expf(-g[e]));
-      du[e] = d[e] * g[e] * s;
-      dg[e] = d[e] * u[e] * s * (1.f + g[e] * (1.f - s));
-    }
+    swiglu_grad8(d, g, u, dg, du);
     *reinterpret_cast<uint4*>(dgate + r * ld_dgu + c) = pack8(dg);
     *reinterpret_cast<uint4*>(dup + r * ld_dgu + c) = pack8(du);
+  }
+}
+// The same gradients with a second, E4M3 output (`fp8_training`): one CTA per row writes dgate / dup in bf16 exactly as
+// swiglu_bwd_kernel does, takes the amax of the rounded [dgate | dup] row, then reads its own bf16 stores back (the
+// same thread wrote them, so plain loads see them) and writes q [rows, 2I] e4m3 (dgate in columns [0, I), dup in
+// [I, 2I)) and s [rows] by the row rule of quant_fp8.py.  No atomics.
+__global__ void __launch_bounds__(256) swiglu_bwd_fp8_kernel(const bf16* __restrict__ dout, const bf16* __restrict__ gate,
+                                                             const bf16* __restrict__ up, bf16* dgate, bf16* dup,
+                                                             uint8_t* __restrict__ q, float* __restrict__ s_out, int I,
+                                                             long long ld_in, long long ld_dout, long long ld_dgu) {
+  __shared__ float red[8];
+  const long long r = blockIdx.x;
+  float a = 0.f;
+  for (int c = threadIdx.x * 8; c < I; c += 256 * 8) {
+    float g[8], u[8], d[8], dg[8], du[8];
+    unpack8(ldg_nc(gate + r * ld_in + c), g);
+    unpack8(ldg_nc(up + r * ld_in + c), u);
+    unpack8(ldg_nc(dout + r * ld_dout + c), d);
+    swiglu_grad8(d, g, u, dg, du);
+    const uint4 pg = pack8(dg), pu = pack8(du);
+    *reinterpret_cast<uint4*>(dgate + r * ld_dgu + c) = pg;
+    *reinterpret_cast<uint4*>(dup + r * ld_dgu + c) = pu;
+    unpack8(pg, dg);
+    unpack8(pu, du);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) a = fmaxf(a, fmaxf(fabsf(dg[e]), fabsf(du[e])));
+  }
+  a = warp_max(a);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = a;
+  __syncthreads();
+  a = red[0];
+#pragma unroll
+  for (int i = 1; i < 8; ++i) a = fmaxf(a, red[i]);
+  if (threadIdx.x == 0) s_out[r] = __fdiv_rn(a, 448.0f);
+  const float rr = fminf(__fdiv_rn(448.0f, a), FLT_MAX);  // amax = 0 or below 448 * 2^-128: +inf -> FLT_MAX
+  uint8_t* qr = q + r * 2 * I;
+  for (int c = threadIdx.x * 8; c < I; c += 256 * 8) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float f[8];
+      unpack8(*reinterpret_cast<const uint4*>((h ? dup : dgate) + r * ld_dgu + c), f);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) f[e] = __fmul_rn(f[e], rr);
+      *reinterpret_cast<uint2*>(qr + h * I + c) = f8_pack8(f);
+    }
   }
 }
 
@@ -839,6 +890,21 @@ int swiglu_bwd_launch(const void* dout, const void* gate, const void* up, void* 
                                                                   (bf16*)dgate, (bf16*)dup, rows, I, ld_in, ld_dout,
                                                                   ld_dgu);
   CB_CUDA_LAUNCH_CHECK("swiglu_bwd");
+  return CB_OK;
+}
+int swiglu_bwd_fp8_launch(const void* dout, const void* gate, const void* up, void* dgate, void* dup, void* q, float* s,
+                          long long rows, int I, long long ld_in, long long ld_dout, long long ld_dgu, cudaStream_t st) {
+  CB_CHECK_ARG(rows > 0 && rows < (1LL << 31) && I > 0 && I % 8 == 0, "swiglu_bwd_fp8: rows=%lld, I=%d must be a "
+               "multiple of 8", rows, I);
+  CB_CHECK_ARG(dout && gate && up && dgate && dup && q && s, "swiglu_bwd_fp8: null argument");
+  CB_CHECK_ARG(ld_in % 8 == 0 && ld_dout % 8 == 0 && ld_dgu % 8 == 0, "swiglu: strides must be multiples of 8");
+  CB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dout) | reinterpret_cast<uintptr_t>(gate) | reinterpret_cast<uintptr_t>(up) |
+                 reinterpret_cast<uintptr_t>(dgate) | reinterpret_cast<uintptr_t>(dup) | reinterpret_cast<uintptr_t>(q)) &
+                15u) == 0, "swiglu_bwd_fp8: every operand must be 16-byte aligned");
+  swiglu_bwd_fp8_kernel<<<(unsigned)rows, 256, 0, st>>>((const bf16*)dout, (const bf16*)gate, (const bf16*)up,
+                                                        (bf16*)dgate, (bf16*)dup, (uint8_t*)q, s, I, ld_in, ld_dout,
+                                                        ld_dgu);
+  CB_CUDA_LAUNCH_CHECK("swiglu_bwd_fp8");
   return CB_OK;
 }
 int rope_launch(void* buf, const long long* pos, const float* cos_t, const float* sin_t, long long rows, int n_heads,

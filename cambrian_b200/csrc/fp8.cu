@@ -24,13 +24,6 @@ namespace cb {
 
 int make_tmap_bf16_3d(CUtensorMap*, const void*, uint64_t, uint64_t, uint64_t, uint64_t, uint64_t, uint32_t);  // gemm.cu
 
-// two fp32 -> two e4m3 (round to nearest even, |x| > 448 -> +-448); lo in the low byte
-__device__ __forceinline__ uint32_t f8_pack2(float lo, float hi) {
-  uint16_t r;
-  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
-  return r;
-}
-
 struct F8Epi {
   const float* sa;      // [M]
   const float* sw;      // [N]

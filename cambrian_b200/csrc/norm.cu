@@ -11,6 +11,7 @@
 // The SVA "latents + pos_embed[window position]" add (vision_sampler.py:304-309) is fused into
 // the LayerNorm load: pos is indexed by the position of the grid cell inside its r x r window.
 #include "common.cuh"
+#include <cfloat>
 
 namespace cb {
 
@@ -44,11 +45,35 @@ __device__ __forceinline__ int pos_index(const PosAdd& p, long long row) {
   return (y % p.r) * p.r + (x % p.r);
 }
 
-template <int TPR, bool RMS>
+template <int TPR>
+__device__ __forceinline__ float row_max(float v, float* red, int row_slot) {
+  v = warp_max(v);
+  if (TPR > 32) {
+    constexpr int W = TPR / 32;
+    const int wid = (threadIdx.x % TPR) >> 5;
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[row_slot * W + wid] = v;
+    __syncthreads();
+    float t = 0.f;
+#pragma unroll
+    for (int i = 0; i < W; ++i) t = fmaxf(t, red[row_slot * W + i]);
+    v = t;
+  }
+  return v;
+}
+
+// E4M3 output of the RMSNorm (F8 = true, `fp8_training`): the row y is rounded to bf16 exactly as the bf16 output is,
+// then quantised by the row rule of quant_fp8.py into q [rows, C] e4m3 and s [rows] fp32; Y is not written
+struct F8Rows {
+  uint8_t* q;
+  float* s;
+};
+
+template <int TPR, bool RMS, bool F8 = false>
 __global__ void __launch_bounds__(TPR < 256 ? 256 : TPR)
 norm_fwd_kernel(const bf16* __restrict__ X, const bf16* __restrict__ gamma, const bf16* __restrict__ beta,
                 bf16* __restrict__ Y, float* __restrict__ mean_out, float* __restrict__ rstd_out,
-                long long rows, int C, float eps, int hf_cast, PosAdd pa) {
+                long long rows, int C, float eps, int hf_cast, PosAdd pa, F8Rows f8 = {}) {
   constexpr int RPB = TPR < 256 ? 256 / TPR : 1;
   __shared__ float red[RPB * (TPR / 32) + 1];
   const int slot = threadIdx.x / TPR, tir = threadIdx.x % TPR;
@@ -92,6 +117,48 @@ norm_fwd_kernel(const bf16* __restrict__ X, const bf16* __restrict__ gamma, cons
     }
     v = row_sum<TPR>(v, red, slot);
     rstd = rsqrtf(v / C + eps);
+  }
+  if constexpr (F8) {
+    static_assert(RMS, "the E4M3 output exists for the RMSNorm only");
+    // y as the bf16 path computes and rounds it, kept in x; then amax, s, r and q of quant_fp8.py
+    const uint4* gp = reinterpret_cast<const uint4*>(gamma);
+    float a = 0.f;
+#pragma unroll
+    for (int i = 0; i < NORM_VPT; ++i) {
+      const int vi = tir + i * TPR;
+      if (active && vi < nvec) {
+        float g[8], o[8];
+        unpack8(gp[vi], g);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          float xh = x[i][e] * rstd;
+          if (hf_cast) xh = __bfloat162float(__float2bfloat16(xh));
+          o[e] = g[e] * xh;
+        }
+        unpack8(pack8(o), x[i]);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) a = fmaxf(a, fabsf(x[i][e]));
+      }
+    }
+    a = row_max<TPR>(a, red, slot);
+    if (!active) return;
+    if (tir == 0) {
+      if (rstd_out) rstd_out[row] = rstd;
+      f8.s[row] = __fdiv_rn(a, 448.0f);
+    }
+    const float r = fminf(__fdiv_rn(448.0f, a), FLT_MAX);  // amax = 0 or below 448 * 2^-128: +inf -> FLT_MAX
+    uint2* qp = reinterpret_cast<uint2*>(f8.q + row * C);
+#pragma unroll
+    for (int i = 0; i < NORM_VPT; ++i) {
+      const int vi = tir + i * TPR;
+      if (vi < nvec) {
+        float t[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) t[e] = __fmul_rn(x[i][e], r);
+        qp[vi] = f8_pack8(t);
+      }
+    }
+    return;
   }
   if (!active) return;
   if (tir == 0) {
@@ -327,6 +394,38 @@ static int norm_bwd_t(const void* dy, const void* x, const void* gamma, const fl
   colsum_kernel<<<(C + 31) / 32, 1024, 0, st>>>(part_g, (int)P, C, (bf16*)dgamma, nullptr);
   if (!RMS && dbeta) colsum_kernel<<<(C + 31) / 32, 1024, 0, st>>>(part_b, (int)P, C, (bf16*)dbeta, nullptr);
   CB_CUDA_LAUNCH_CHECK("norm_bwd colsum");
+  return CB_OK;
+}
+
+// RMSNorm forward with an E4M3 output (`fp8_training`): the pick_tpr / row layout of norm_fwd_t, so rstd and the bf16
+// rounding of y match rmsnorm_fwd bit for bit; q [rows, C] e4m3, s [rows] fp32 by the quant_fp8.py row rule
+int rmsnorm_fwd_fp8(const void* x, const void* gamma, void* q, float* s, float* rstd, long long rows, int C, float eps,
+                    int hf_cast, cudaStream_t st) {
+  const int tpr = pick_tpr(C);
+  CB_CHECK_ARG(C % 16 == 0 && tpr != 0, "rmsnorm_fwd_fp8: C=%d must be a multiple of 16 and <= 16384", C);
+  CB_CHECK_ARG(rows > 0, "rmsnorm_fwd_fp8: rows=%lld", rows);
+  CB_CHECK_ARG(x && gamma && q && s, "rmsnorm_fwd_fp8: null argument");
+  CB_CHECK_ARG(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(q)) &
+                15u) == 0, "rmsnorm_fwd_fp8: x, gamma and q must be 16-byte aligned");
+  const PosAdd pa{nullptr, 1, 1};
+  const F8Rows f8{(uint8_t*)q, s};
+#define CB_NORM_FWD_F8(T)                                                                                     \
+  {                                                                                                           \
+    constexpr int RPB = T < 256 ? 256 / T : 1;                                                                \
+    const unsigned grid = (unsigned)((rows + RPB - 1) / RPB);                                                 \
+    norm_fwd_kernel<T, true, true><<<grid, T < 256 ? 256 : T, 0, st>>>((const bf16*)x, (const bf16*)gamma,    \
+                                                                      nullptr, nullptr, nullptr, rstd, rows, C, \
+                                                                      eps, hf_cast, pa, f8);                   \
+  }
+  switch (tpr) {
+    case 32: CB_NORM_FWD_F8(32) break;
+    case 64: CB_NORM_FWD_F8(64) break;
+    case 128: CB_NORM_FWD_F8(128) break;
+    case 256: CB_NORM_FWD_F8(256) break;
+    default: CB_NORM_FWD_F8(512) break;
+  }
+#undef CB_NORM_FWD_F8
+  CB_CUDA_LAUNCH_CHECK("rmsnorm_fwd_fp8");
   return CB_OK;
 }
 

@@ -25,7 +25,7 @@ try:  # transformers >= 5: initialisers that honour the per-parameter `_is_hf_in
 except ImportError:  # pragma: no cover - older transformers
     _hf_init = None
 
-from ... import ops
+from ... import ops, train_fp8
 from ...autograd import DecoderLayerFn, LinearFn, LMHeadLossFn, RMSNormFn, SpanMergeFn, SpanSplitFn
 from ..cambrian_arch import IGNORE_INDEX, CambrianMetaForCausalLM, CambrianMetaModel, WindowedFeatures
 
@@ -182,9 +182,12 @@ class CBLlamaDecoderLayer(nn.Module):
             return self.infer(x, rt, None)
         a, m = self.self_attn, self.mlp
         qkv_w, gu_w, g_qkv, g_gu = self._fused()
+        fp8 = bool(rt.get("fp8", False))
+        if fp8:
+            train_fp8.check_widths(x.shape[-1], gu_w.shape[0] // 2, qkv_w.shape[0])
         meta = dict(nh=self.nh, nkv=self.nkv, hd=self.hd, eps=self.input_layernorm.variance_epsilon,
                     hf_cast=rt["hf_cast"], cos=rt["cos"], sin=rt["sin"], pos=rt["pos"], kmask=rt["kmask"],
-                    recompute=rt["recompute"], qkv_w=qkv_w, gu_w=gu_w,
+                    recompute=rt["recompute"], fp8=fp8, qkv_w=qkv_w, gu_w=gu_w,
                     params=(self.input_layernorm.weight, g_qkv, a.o_proj.weight, self.post_attention_layernorm.weight,
                             g_gu, m.down_proj.weight))
         return DecoderLayerFn.apply(meta, x, self.input_layernorm.weight, a.q_proj.weight, a.k_proj.weight,
@@ -385,7 +388,7 @@ class CambrianLlamaModel(CambrianMetaModel, CBLlamaModel):
         elif attention_mask is not None:
             kmask = attention_mask.bool().contiguous()
         rt = dict(pos=pos, cos=cos, sin=sin, kmask=kmask, hf_cast=not self.training,
-                  recompute=bool(self.gradient_checkpointing and self.training))
+                  recompute=bool(self.gradient_checkpointing and self.training), fp8=train_fp8.enabled(cfg))
         sites = []
         if not getattr(cfg, "connector_only", True) and vision_tower_aux_feature_list is not None:
             sites = [cfg.start_of_vision_sampler_layers + k * cfg.stride_of_vision_sampler_layers

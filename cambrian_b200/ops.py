@@ -943,6 +943,57 @@ def fp8_mlp_gate_up(h2d, qw):
 
 
 # ------------------------------------------------------------------------------------------------
+# FP8 E4M3 training of the decoder projections (fp8_training; the format lives in train_fp8.py)
+# ------------------------------------------------------------------------------------------------
+def fp8_quantize_weight_t(w, wtq, st):
+    """Quantise the transpose of one bf16 [N, K] weight (contiguous rows, any row stride) into caller-allocated
+    wtq float8_e4m3fn [K, N] and st fp32 [K]: bit for bit fp8_quantize_weight(w.t().contiguous())."""
+    _require_cuda_bf16(w)
+    N, K = w.shape
+    if (w.stride(1) != 1 or wtq.shape != (K, N) or not wtq.is_contiguous() or wtq.dtype != torch.float8_e4m3fn
+            or st.shape != (K,) or st.dtype != torch.float32):
+        raise ValueError("fp8_quantize_weight_t: need w [N, K] with contiguous rows, wtq float8_e4m3fn [K, N], st fp32 [K]")
+    lib = _lib.load()
+    ws = workspace(max(int(lib.cb_fp8_quantize_weight_t_workspace_floats(N, K)), 1), w.device)
+    check(lib.cb_fp8_quantize_weight_t(ptr(w), N, K, w.stride(0), ptr(wtq), ptr(st), ptr(ws), ws.numel(), stream()),
+          "cb_fp8_quantize_weight_t")
+
+
+def rmsnorm_fwd_fp8(x, gamma, eps: float = 1e-6, hf_cast: bool = False):
+    """rmsnorm_fwd with an E4M3 output: x [rows, C] -> ((xq float8_e4m3fn [rows, C], sa fp32 [rows]), rstd fp32 [rows]),
+    bit for bit fp8_quantize_act(rmsnorm_fwd(x)) and rmsnorm_fwd's rstd; the bf16 y is not written."""
+    _require_cuda_bf16(x, gamma)
+    C_ = x.shape[-1]
+    if not x.is_contiguous() or gamma.shape != (C_,):
+        raise ValueError("rmsnorm_fwd_fp8: x must be contiguous and gamma [C]")
+    x2 = x.reshape(-1, C_)
+    rows = x2.shape[0]
+    xq = torch.empty((rows, C_), dtype=torch.float8_e4m3fn, device=x.device)
+    sa = torch.empty(rows, dtype=torch.float32, device=x.device)
+    rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
+    check(_lib.load().cb_rmsnorm_fwd_fp8(ptr(x2), ptr(gamma), ptr(xq), ptr(sa), ptr(rstd), rows, C_, float(eps),
+                                         int(hf_cast), stream()), "cb_rmsnorm_fwd_fp8")
+    return (xq, sa), rstd
+
+
+def swiglu_bwd_fp8(dout, gate, up, dgate, dup):
+    """swiglu_bwd (dgate / dup written as swiglu_bwd writes them) plus the E4M3 rows of [dgate | dup]: returns
+    (dguq float8_e4m3fn [rows, 2I], sdgu fp32 [rows]), bit for bit fp8_quantize_act of the bf16 [rows, 2I] gradient."""
+    _require_cuda_bf16(dout, gate, up, dgate, dup)
+    rows, I = gate.shape
+    if (up.shape != (rows, I) or dout.shape != (rows, I) or dgate.shape != (rows, I) or dup.shape != (rows, I)
+            or gate.stride(0) != up.stride(0) or dgate.stride(0) != dup.stride(0)
+            or any(t.stride(1) != 1 for t in (dout, gate, up, dgate, dup))):
+        raise ValueError("swiglu_bwd_fp8: need [rows, I] views with contiguous rows, gate / up and dgate / dup each at "
+                         "one common row stride")
+    dguq = torch.empty((rows, 2 * I), dtype=torch.float8_e4m3fn, device=gate.device)
+    sdgu = torch.empty(rows, dtype=torch.float32, device=gate.device)
+    check(_lib.load().cb_swiglu_bwd_fp8(ptr(dout), ptr(gate), ptr(up), ptr(dgate), ptr(dup), ptr(dguq), ptr(sdgu), rows,
+                                        I, gate.stride(0), dout.stride(0), dgate.stride(0), stream()), "cb_swiglu_bwd_fp8")
+    return dguq, sdgu
+
+
+# ------------------------------------------------------------------------------------------------
 # FP8 E4M3 decode KV cache (kv_cache_dtype="fp8"; the format and the decode arithmetic live in kv_fp8.py)
 # ------------------------------------------------------------------------------------------------
 def kv_fp8_append(k, v, kq, vq, ks, vs, offset: int = 0, offset_dev=None):

@@ -348,6 +348,28 @@ int cb_attn_decode_fp8(const void* q, int64_t q_bs, const void* kq, const void* 
                        const void* kmask, int64_t kmask_ld, void* o, float* workspace, int64_t workspace_floats, int B, int Sq,
                        int nh, int nkv, int S_max, int hd, int64_t length, const int64_t* length_dev, float scale,
                        void* stream);
+/* FP8 E4M3 training of the decoder projections (`config.fp8_training`; the format is defined in
+ * cambrian_b200/train_fp8.py).  The four forward GEMMs (y = x W^T) and the four input-gradient GEMMs (dx = dy W) of a
+ * decoder layer run on cb_gemm_fp8 with the row rule above; the weight-gradient GEMMs stay bf16.  Every scale is constant
+ * along the reduction dimension: per token on the activation / gradient side, per row of W in forward and per row of
+ * W^T (per input column of W) in the input-gradient GEMM.
+ *
+ * cb_fp8_quantize_weight_t: bf16 W [N, K] (row stride ldw) -> wtq e4m3 [K, N] (row stride N), st fp32 [K], bit for bit
+ * cb_fp8_quantize_weight of W^T; N % 16 == 0, K % 16 == 0.  Column maxima go through `workspace` (at least
+ * cb_fp8_quantize_weight_t_workspace_floats(N, K) floats on the current device); no atomics. */
+int64_t cb_fp8_quantize_weight_t_workspace_floats(int N, int K);
+int cb_fp8_quantize_weight_t(const void* w, int N, int K, int64_t ldw, void* wtq, float* st, float* workspace,
+                             int64_t workspace_floats, void* stream);
+/* cb_rmsnorm_fwd with an E4M3 output: y is computed and rounded to bf16 as cb_rmsnorm_fwd does, then quantised per row
+ * into xq e4m3 [rows, C] and sa fp32 [rows]; rstd [rows] as cb_rmsnorm_fwd writes it (may be NULL).  Bit for bit
+ * cb_fp8_quantize_act(cb_rmsnorm_fwd(x)).  C % 16 == 0. */
+int cb_rmsnorm_fwd_fp8(const void* x, const void* gamma, void* xq, float* sa, float* rstd, int64_t rows, int C, float eps,
+                       int hf_cast, void* stream);
+/* cb_swiglu_bwd with a second output: dgate / dup bf16 exactly as cb_swiglu_bwd writes them, plus dguq e4m3 [rows, 2I]
+ * (contiguous; dgate in columns [0, I), dup in [I, 2I)) and sdgu fp32 [rows] by the row rule over the whole [dgate | dup]
+ * row: bit for bit cb_fp8_quantize_act of the [rows, 2I] gradient.  I % 8 == 0; one CTA per row, no atomics. */
+int cb_swiglu_bwd_fp8(const void* dout, const void* gate, const void* up, void* dgate, void* dup, void* dguq, float* sdgu,
+                      int64_t rows, int I, int64_t ld_in, int64_t ld_dout, int64_t ld_dgu, void* stream);
 
 #ifdef __cplusplus
 }
