@@ -72,6 +72,8 @@ def load_pretrained_model(model_path, model_base=None, model_name="cambrian", lo
                           device="cuda", dtype=torch.bfloat16, load_tokenizer=True, load_fp8=False, **kwargs):
     """model/builder.py:29-175 for the LLaMA-family Cambrian checkpoints: returns (tokenizer, model, image_processor list,
     context_len).  `model_base` + `<model_path>/mm_projector.bin` is the connector-only layout (:103-114).
+    A `phi3` model name loads Cambrian-Phi3 (cambrian_phi3.py) in bf16 with the fast tokenizer (:109-115); the weight
+    formats are LLaMA-only and raise NotImplementedError for it.
     load_4bit=True (:37-44): the checkpoint loads in bf16 on the CPU, the seven projections of every decoder layer are
     quantised to NF4 layer by layer on `device` (quant.quantize_decoder_nf4_), everything else moves there in bf16.
     load_8bit=True (:35-36) does the same with LLM.int8 weights (quant_int8.quantize_decoder_int8_) and takes precedence
@@ -90,8 +92,10 @@ def load_pretrained_model(model_path, model_base=None, model_name="cambrian", lo
         raise NotImplementedError("8-bit (LLM.int8) weights run on CUDA only and no CUDA device is available")
     if "lora" in model_name.lower():
         raise NotImplementedError("LoRA merging (builder.py:56-92) is outside the hot path: merge with the reference tools first")
-    if "mistral" in model_name.lower() or "phi3" in model_name.lower():
+    if "mistral" in model_name.lower():
         raise NotImplementedError("only the LLaMA-family Cambrian models (8B / 13B / 34B) are implemented")
+    if "phi3" in model_name.lower():
+        return _load_phi3(model_path, model_base, load_8bit, load_4bit, load_fp8, device, dtype, load_tokenizer, **kwargs)
     tok_src = model_base if model_base is not None else model_path
     tokenizer = AutoTokenizer.from_pretrained(tok_src, use_fast=False) if load_tokenizer else None
     if model_base is not None:
@@ -110,6 +114,31 @@ def load_pretrained_model(model_path, model_base=None, model_name="cambrian", lo
         from .quant import quantize_decoder_nf4_
         quantize_decoder_nf4_(model, device)
     model.to(device=device, dtype=dtype)
+    return _finish(tokenizer, model, device, dtype)
+
+
+def _load_phi3(model_path, model_base, load_8bit, load_4bit, load_fp8, device, dtype, load_tokenizer, **kwargs):
+    """model/builder.py:109-115: Cambrian-Phi3 (CambrianPhi3ForCausalLM) with the fast AutoTokenizer, in bf16."""
+    from transformers import AutoConfig, AutoTokenizer
+
+    from .model.language_model.cambrian_phi3 import CambrianPhi3ForCausalLM
+    if load_4bit or load_8bit or load_fp8:
+        fmt = "load_fp8" if load_fp8 else "load_8bit" if load_8bit else "load_4bit"
+        raise NotImplementedError(f"Cambrian-Phi3 with {fmt}: the weight quantisers address the LLaMA projections "
+                                  "(q_proj ... down_proj) by name, not Phi-3's fused qkv_proj / gate_up_proj; load it in bf16")
+    tok_src = model_base if model_base is not None else model_path
+    tokenizer = AutoTokenizer.from_pretrained(tok_src) if load_tokenizer else None
+    if model_base is not None:
+        cfg = AutoConfig.from_pretrained(model_path)
+        model = CambrianPhi3ForCausalLM.from_pretrained(model_base, config=cfg, torch_dtype=dtype, **kwargs)
+        load_mm_projector(model, os.path.join(model_path, "mm_projector.bin"))
+    else:
+        model = CambrianPhi3ForCausalLM.from_pretrained(model_path, torch_dtype=dtype, **kwargs)
+    model.to(device=device, dtype=dtype)
+    return _finish(tokenizer, model, device, dtype)
+
+
+def _finish(tokenizer, model, device, dtype):
     towers = model.get_vision_tower_aux_list() or []
     for t in towers:
         if not t.is_loaded:

@@ -53,7 +53,7 @@ long long norm_bwd_workspace_floats(long long, int);
 
 int attn_fwd_launch(const void*, const void*, const void*, void*, float*, const void*, int, int, int, int, int, int,
                     long long, long long, long long, long long, long long, long long, long long, long long, float, int,
-                    cudaStream_t);
+                    int, cudaStream_t);
 int attn_bwd_launch(const void*, const void*, const void*, const void*, const void*, const float*, float*, void*, void*,
                     void*, const void*, int, int, int, int, int, int, long long, long long, long long, long long,
                     long long, long long, long long, long long, long long, long long, long long, long long, long long,
@@ -195,7 +195,14 @@ int cb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse
                 int nkv, int Sq, int Skv, int hd, int64_t q_bs, int64_t q_ss, int64_t k_bs, int64_t k_ss,
                 int64_t v_bs, int64_t v_ss, int64_t o_bs, int64_t o_ss, float scale, int causal, void* stream) {
   return cb::attn_fwd_launch(q, k, v, o, lse, kmask, B, nh, nkv, Sq, Skv, hd, q_bs, q_ss, k_bs, k_ss, v_bs, v_ss, o_bs,
-                             o_ss, scale, causal, ST(stream));
+                             o_ss, scale, causal, 0, ST(stream));
+}
+int cb_attn_fwd_window(const void* q, const void* k, const void* v, void* o, float* lse, const void* kmask, int B,
+                       int nh, int nkv, int Sq, int Skv, int hd, int64_t q_bs, int64_t q_ss, int64_t k_bs, int64_t k_ss,
+                       int64_t v_bs, int64_t v_ss, int64_t o_bs, int64_t o_ss, float scale, int causal, int window,
+                       void* stream) {
+  return cb::attn_fwd_launch(q, k, v, o, lse, kmask, B, nh, nkv, Sq, Skv, hd, q_bs, q_ss, k_bs, k_ss, v_bs, v_ss, o_bs,
+                             o_ss, scale, causal, window, ST(stream));
 }
 int cb_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                 float* delta, void* dq, void* dk, void* dv, const void* kmask, int B, int nh, int nkv, int Sq,

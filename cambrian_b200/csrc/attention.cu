@@ -41,6 +41,8 @@ struct AttnParams {
   const uint8_t* kmask;  // [B, Skv] 1 = attend, may be null
   int B, nh, nkv, Sq, Skv, hd, causal;
   float scale_log2;      // softmax scale * log2(e)
+  int window;            // sliding window (attn_fwd_kernel<HDP, true>): key slot j is visible from query slot i iff
+                         // 0 <= i - j < window
 };
 
 // true iff every key of [k0, k0 + N) is set in the key mask (the caller checks k0 + N <= Skv): N / 32 bytes per lane in
@@ -82,7 +84,10 @@ struct FwdCfg {
   static constexpr int SMEM = TILE * (1 + 2 * STAGES) + 1024 + 256;
 };
 
-template <int HDP>
+// WIN: causal sliding-window attention (p.window > 0).  Key tiles that lie wholly before the window of every row of a
+// consumer warpgroup are skipped (the producer does not load the ones before the CTA's first row's window); tiles on the
+// window's edge take the per-element path.  WIN = false compiles to the plain causal / non-causal kernel.
+template <int HDP, bool WIN>
 __global__ void __launch_bounds__(288, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, AttnParams p) {
@@ -115,6 +120,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     n_tiles = min(kv_tiles_all, last_key / 128 + 1);
     if (n_tiles < 1) n_tiles = 1;
   }
+  // first key tile inside the window of the CTA's first query row (slot q0 + coff sees keys from q0 + coff - window + 1)
+  int j_lo = 0;
+  if (WIN) j_lo = min(n_tiles - 1, max(0, q0 + coff - p.window + 1) / 128);
 
   if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmQ);
@@ -138,7 +146,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       for (int a = 0; a < Cfg::ATOMS; ++a) tma_load_4d(sQ + a * 16384, &tmQ, q_full, a * 64, h, q0, b);
       int st = 0;
       uint32_t ph = 0;
-      for (int j = 0; j < n_tiles; ++j) {
+      for (int j = j_lo; j < n_tiles; ++j) {
         mbar_wait(kv_empty(st), ph ^ 1u);
         mbar_arrive_expect_tx(k_full(st), Cfg::TILE);
 #pragma unroll
@@ -167,10 +175,18 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   mbar_wait(q_full, 0);
   int st = 0;
   uint32_t ph = 0;
-  for (int j = 0; j < n_tiles; ++j) {
+  for (int j = j_lo; j < n_tiles; ++j) {
     const int k0 = j * 128;
     float s[64];
     mbar_wait(k_full(st), ph);
+    if (WIN && k0 + 127 < q0 + wg * 64 + coff - p.window + 1) {
+      // before the window of all 64 rows of this warpgroup: nothing to compute.  Waiting for V as well keeps the stage's
+      // barrier phases in step with the producer before the slot is released.
+      mbar_wait(v_full(st), ph);
+      if (wg_leader) mbar_arrive(kv_empty(st));
+      if (++st == STAGES) { st = 0; ph ^= 1u; }
+      continue;
+    }
     const uint32_t kb = sK + st * Cfg::TILE;
     wgmma_fence();
 #pragma unroll
@@ -183,6 +199,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     // masking (keys past Skv, past the diagonal, padded keys) -> -inf; scores into the log2 domain.  A tile inside Skv,
     // below the diagonal for all 64 rows of the warpgroup, whose keys are all valid keeps every score as it is.
     bool full_tile = k0 + 128 <= p.Skv && (!p.causal || k0 + 127 <= q0 + wg * 64 + coff);
+    if (WIN) full_tile = full_tile && k0 + p.window > q0 + wg * 64 + 63 + coff;  // inside the last row's window too
     if (full_tile && km) full_tile = keys_all_valid<128>(km, k0);
     wgmma_wait<0>();
     reg_fence(s);
@@ -195,7 +212,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         if (!full_tile) {
           const int key = k0 + 8 * jj + cq + (e & 1);
           const int qi = q0 + rloc + 8 * (e >> 1);
-          const bool ok = key < p.Skv && (!p.causal || key <= qi + coff) && (!km || km[key]);
+          const bool ok = key < p.Skv && (!p.causal || key <= qi + coff) && (!km || km[key]) &&
+                          (!WIN || qi + coff - key < p.window);
           v = ok ? v : -INFINITY;
         }
         s[4 * jj + e] = v;
@@ -738,11 +756,11 @@ int make_tmap_bf16_4d(CUtensorMap* out, const void* base, uint64_t d0, uint64_t 
 
 static int hd_padded(int hd) { return (hd + 15) / 16 * 16; }
 
-template <int HDP>
+template <int HDP, bool WIN>
 static int launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnParams& p,
                       cudaStream_t st) {
   using Cfg = FwdCfg<HDP>;
-  auto kern = attn_fwd_kernel<HDP>;
+  auto kern = attn_fwd_kernel<HDP, WIN>;
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
@@ -757,8 +775,9 @@ static int launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtens
 int attn_fwd_launch(const void* q, const void* k, const void* v, void* o, float* lse, const void* kmask, int B,
                     int nh, int nkv, int Sq, int Skv, int hd, long long q_bs, long long q_ss, long long k_bs,
                     long long k_ss, long long v_bs, long long v_ss, long long o_bs, long long o_ss, float scale,
-                    int causal, cudaStream_t st) {
+                    int causal, int window, cudaStream_t st) {
   CB_CHECK_ARG(B > 0 && nh > 0 && nkv > 0 && Sq > 0 && Skv > 0, "attention: empty problem");
+  CB_CHECK_ARG(window >= 0 && (window == 0 || causal), "attention: window=%d needs causal attention (0 = none)", window);
   CB_CHECK_ARG(nh % nkv == 0, "attention: nh=%d not a multiple of nkv=%d", nh, nkv);
   CB_CHECK_ARG(hd % 8 == 0 && hd <= 128, "attention: head_dim=%d must be a multiple of 8 and <= 128", hd);
   CB_CHECK_ARG(o_ss % 8 == 0 && o_bs % 8 == 0 && !(reinterpret_cast<uintptr_t>(o) & 15u),
@@ -772,11 +791,19 @@ int attn_fwd_launch(const void* q, const void* k, const void* v, void* o, float*
   p.o = (bf16*)o; p.o_bs = o_bs; p.o_ss = o_ss; p.lse = lse; p.kmask = (const uint8_t*)kmask;
   p.B = B; p.nh = nh; p.nkv = nkv; p.Sq = Sq; p.Skv = Skv; p.hd = hd; p.causal = causal;
   p.scale_log2 = scale * LOG2E;
+  p.window = window;
   const int hdp = hd_padded(hd);
-  if (hdp <= 64) return launch_fwd<64>(tq, tk, tv, p, st);
-  if (hdp <= 80) return launch_fwd<80>(tq, tk, tv, p, st);
-  if (hdp <= 96) return launch_fwd<96>(tq, tk, tv, p, st);
-  return launch_fwd<128>(tq, tk, tv, p, st);
+  // the largest query-key distance is Skv - 1: a window of Skv or more hides nothing and takes the plain kernel
+  if (window > 0 && window < Skv) {
+    if (hdp <= 64) return launch_fwd<64, true>(tq, tk, tv, p, st);
+    if (hdp <= 80) return launch_fwd<80, true>(tq, tk, tv, p, st);
+    if (hdp <= 96) return launch_fwd<96, true>(tq, tk, tv, p, st);
+    return launch_fwd<128, true>(tq, tk, tv, p, st);
+  }
+  if (hdp <= 64) return launch_fwd<64, false>(tq, tk, tv, p, st);
+  if (hdp <= 80) return launch_fwd<80, false>(tq, tk, tv, p, st);
+  if (hdp <= 96) return launch_fwd<96, false>(tq, tk, tv, p, st);
+  return launch_fwd<128, false>(tq, tk, tv, p, st);
 }
 
 template <int HDP>

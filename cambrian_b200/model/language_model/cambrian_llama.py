@@ -149,6 +149,8 @@ class CBLlamaMLP(nn.Module):
 
 
 class CBLlamaDecoderLayer(nn.Module):
+    window = 0                  # causal sliding window of the attention (0: none); Phi-3's layer sets it
+
     def __init__(self, config, layer_idx):
         super().__init__()
         self.layer_idx = layer_idx
@@ -213,13 +215,15 @@ class CBLlamaDecoderLayer(nn.Module):
         q = qkv[:, : nh * hd].view(B, S, nh, hd)
         k_new = qkv[:, nh * hd:(nh + nkv) * hd].view(B, S, nkv, hd)
         v_new = qkv[:, (nh + nkv) * hd:].view(B, S, nkv, hd)
+        win = {"window": self.window} if self.window else {}
         if cache is None:
-            attn = ops.attn_fwd(q, k_new, v_new, causal=True, kmask=rt["kmask"])
+            attn = ops.attn_fwd(q, k_new, v_new, causal=True, kmask=rt["kmask"], **win)
         elif cache.fp8 is not None:
             attn = self._attn_fp8_cache(q, k_new, v_new, cache, rt["kmask"])
         elif cache.slot is not None:
             # static-shape decode step (CUDA-graph replay): the write slot is a DEVICE index, attention runs over the whole
-            # cache buffer and the validity mask (updated on the device) hides the slots not written yet
+            # cache buffer and the validity mask (updated on the device) hides the slots not written yet and, with a
+            # sliding window, the ones that have left it
             kc, vc = cache.k[self.layer_idx], cache.v[self.layer_idx]
             kc.index_copy_(1, cache.slot, k_new)
             vc.index_copy_(1, cache.slot, v_new)
@@ -229,7 +233,7 @@ class CBLlamaDecoderLayer(nn.Module):
             t0 = cache.length
             kc[:, t0:t0 + S].copy_(k_new)   # cache append (memory plumbing)
             vc[:, t0:t0 + S].copy_(v_new)
-            attn = ops.attn_fwd(q, kc[:, : t0 + S], vc[:, : t0 + S], causal=True, kmask=rt["kmask"])
+            attn = ops.attn_fwd(q, kc[:, : t0 + S], vc[:, : t0 + S], causal=True, kmask=rt["kmask"], **win)
         attn2 = attn.view(rows, nh * hd)
         if qp is not None:
             x1 = qp["o"].linear(attn2, residual=x2)
@@ -331,12 +335,14 @@ class CambrianPreTrainedModel(PreTrainedModel):
 
 
 class CBLlamaModel(CambrianPreTrainedModel):
+    decoder_layer_cls = CBLlamaDecoderLayer
+
     def __init__(self, config):
         super().__init__(config)
         self.padding_idx = getattr(config, "pad_token_id", None)
         self.vocab_size = config.vocab_size
         self.embed_tokens = nn.Embedding(config.vocab_size, config.hidden_size, self.padding_idx)
-        self.layers = nn.ModuleList([CBLlamaDecoderLayer(config, i) for i in range(config.num_hidden_layers)])
+        self.layers = nn.ModuleList([self.decoder_layer_cls(config, i) for i in range(config.num_hidden_layers)])
         self.norm = CBRMSNorm(config.hidden_size, eps=config.rms_norm_eps)
         self.gradient_checkpointing = False
         self._rope = None
@@ -477,6 +483,10 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
 
     def get_model(self):
         return self.model
+
+    def attention_window(self) -> int:
+        """Causal sliding window of the decoder's attention (0: none)."""
+        return 0
 
     def save_pretrained(self, *args, **kwargs):
         from ...quant import quantized_format
@@ -653,12 +663,18 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
         tok_buf = torch.zeros(B, dtype=torch.long, device=dev)
         logits_buf = torch.empty((B, self.lm_head.weight.shape[0]), dtype=torch.float32, device=dev)
         cache.slot = torch.full((1,), cache.length, dtype=torch.long, device=dev)
+        window = self.attention_window()
 
         def step():
             ops.gemm(h_buf, self.lm_head.weight, out=logits_buf)                                 # fp32 logits (:409)
             nxt = logits_buf.argmax(-1)
             tok_buf.copy_(torch.where(done_buf, torch.full_like(nxt, pad), nxt))
             cache.kmask.index_fill_(1, cache.slot, True)
+            if window:
+                # the query at slot s sees slots s - window + 1 .. s: slot s - window leaves the window now (nothing
+                # leaves while s < window); an index and a select-and-mask on the device, no host sync
+                old = (cache.slot - window).clamp_(min=0)
+                cache.kmask.index_copy_(1, old, cache.kmask.index_select(1, old) & (cache.slot < window))
             out = self.model(input_ids=tok_buf.view(B, 1), position_ids=pos_buf, past_key_values=cache, use_cache=True)
             h_buf.copy_(out.last_hidden_state[:, 0])
             pos_buf.add_(1)
@@ -666,6 +682,8 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
 
         # slots beyond the prompt start invalid; each step validates the one it writes
         cache.kmask[:, S0:] = False
+        if window:
+            cache.kmask[:, :max(0, S0 - window)] = False    # already outside the first step's window
         snap = (h_buf.clone(), pos_buf.clone(), cache.slot.clone(), cache.kmask.clone())
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream())

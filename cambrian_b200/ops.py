@@ -288,8 +288,11 @@ def _bshd_strides(t, hd):
     return t.stride(0), t.stride(1)
 
 
-def attn_fwd(q, k, v, *, causal: bool, kmask=None, scale: float | None = None, need_lse: bool = False, out=None):
-    """q [B,Sq,nh,hd], k/v [B,Skv,nkv,hd] (views are fine) -> o [B,Sq,nh,hd] contiguous (+ lse [B,nh,Sq])."""
+def attn_fwd(q, k, v, *, causal: bool, kmask=None, scale: float | None = None, need_lse: bool = False, out=None,
+             window: int = 0):
+    """q [B,Sq,nh,hd], k/v [B,Skv,nkv,hd] (views are fine) -> o [B,Sq,nh,hd] contiguous (+ lse [B,nh,Sq]).
+    window > 0 (causal only): query slot i = row + Skv - Sq sees key slot j iff 0 <= i - j < window (Phi-3's sliding
+    window as transformers' `_prepare_4d_causal_attention_mask` builds it)."""
     _require_cuda_bf16(q, k, v)
     B, Sq, nh, hd = q.shape
     Skv, nkv = k.shape[1], k.shape[2]
@@ -304,6 +307,12 @@ def attn_fwd(q, k, v, *, causal: bool, kmask=None, scale: float | None = None, n
     if kmask is not None:
         kmask = kmask.contiguous()
         kmask = kmask.view(torch.uint8) if kmask.dtype == torch.bool else kmask.to(torch.uint8)
+    if window:
+        rc = _lib.load().cb_attn_fwd_window(ptr(q), ptr(k), ptr(v), ptr(o), ptr(lse), ptr(kmask), B, nh, nkv, Sq, Skv,
+                                            hd, qb, qs, kb, ks, vb, vs_, ob, os_, float(scale), int(causal), int(window),
+                                            stream())
+        check(rc, "cb_attn_fwd_window")
+        return (o, lse) if need_lse else o
     rc = _lib.load().cb_attn_fwd(ptr(q), ptr(k), ptr(v), ptr(o), ptr(lse), ptr(kmask), B, nh, nkv, Sq, Skv, hd,
                                  qb, qs, kb, ks, vb, vs_, ob, os_, float(scale), int(causal), stream())
     check(rc, "cb_attn_fwd")

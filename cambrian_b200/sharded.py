@@ -28,6 +28,9 @@ class Zero3Inference:
     def __init__(self, model, process_group=None):
         """`model`: a CambrianLlamaForCausalLM already on its device in bf16 (full weights are dropped layer by layer
         as they are sharded; load on CPU / meta and move layer-wise for models that do not fit one GPU)."""
+        if getattr(model.config, "model_type", None) == "cambrian_phi3":
+            raise NotImplementedError("Zero3Inference does not shard Cambrian-Phi3: its layer layout (fused qkv_proj / "
+                                      "gate_up_proj) is not the LLaMA one it streams; the 3B model runs on one GPU")
         from .quant import quantized_format
         fmt = quantized_format(model)
         if fmt is not None:

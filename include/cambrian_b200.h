@@ -107,6 +107,13 @@ int64_t cb_norm_bwd_workspace_floats(int64_t rows, int C);
 int cb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, const void* kmask, int B, int nh,
                 int nkv, int Sq, int Skv, int hd, int64_t q_bs, int64_t q_ss, int64_t k_bs, int64_t k_ss,
                 int64_t v_bs, int64_t v_ss, int64_t o_bs, int64_t o_ss, float scale, int causal, void* stream);
+/* cb_attn_fwd with a causal sliding window (Phi-3): key slot j is visible from query slot i (i = query row + Skv - Sq)
+ * iff 0 <= i - j < window, on top of the key mask.  window = 0 means none and is cb_attn_fwd exactly; window > 0 needs
+ * causal = 1.  Key tiles before the window of a whole warpgroup are skipped, not masked. */
+int cb_attn_fwd_window(const void* q, const void* k, const void* v, void* o, float* lse, const void* kmask, int B,
+                       int nh, int nkv, int Sq, int Skv, int hd, int64_t q_bs, int64_t q_ss, int64_t k_bs, int64_t k_ss,
+                       int64_t v_bs, int64_t v_ss, int64_t o_bs, int64_t o_ss, float scale, int causal, int window,
+                       void* stream);
 /* delta [B, nh, Sq] fp32 scratch; dq/dk/dv written (bf16, strided, heads packed at hd: dq may be a view into a packed
  * dQKV buffer).  Every output element has one writer (no atomics), so the results are bit-identical from run to run. */
 int cb_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
