@@ -36,6 +36,7 @@ SIGNATURES = {
     "cb_attn_fwd": (_i, [_vp] * 6 + [_i] * 6 + [_i64] * 8 + [_f, _i, _vp]),
     "cb_attn_fwd_window": (_i, [_vp] * 6 + [_i] * 6 + [_i64] * 8 + [_f, _i, _i, _vp]),
     "cb_attn_bwd": (_i, [_vp] * 11 + [_i] * 6 + [_i64] * 16 + [_f, _i, _vp]),
+    "cb_attn_bwd_window": (_i, [_vp] * 11 + [_i] * 6 + [_i64] * 16 + [_f, _i, _i, _vp]),
     "cb_act_fwd": (_i, [_vp, _vp, _i64, _i, _vp]),
     "cb_act_bwd": (_i, [_vp, _vp, _vp, _i64, _i, _vp]),
     "cb_swiglu_fwd": (_i, [_vp, _vp, _vp, _i64, _i, _i64, _i64, _vp]),

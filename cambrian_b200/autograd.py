@@ -612,7 +612,8 @@ class DecoderLayerFn(torch.autograd.Function):
 
     meta = dict(nh, nkv, hd, eps, hf_cast, cos, sin, pos (int64 [B*S]), kmask (bool [B,S] or None), params (6 Parameters),
                 recompute (bool: keep only x and redo the forward in backward — per-layer activation checkpointing),
-                fp8 (bool, optional: the four projection GEMMs and their input-gradient GEMMs in E4M3, train_fp8.py))
+                fp8 (bool, optional: the four projection GEMMs and their input-gradient GEMMs in E4M3, train_fp8.py),
+                window (int, optional: causal sliding window of the attention, 0 = none; Phi-3))
     """
 
     @staticmethod
@@ -633,7 +634,8 @@ class DecoderLayerFn(torch.autograd.Function):
         q = qkv[:, : nh * hd].view(B, S, nh, hd)
         k = qkv[:, nh * hd:(nh + nkv) * hd].view(B, S, nkv, hd)
         v = qkv[:, (nh + nkv) * hd:].view(B, S, nkv, hd)
-        attn, lse = ops.attn_fwd(q, k, v, causal=True, kmask=meta["kmask"], need_lse=True)
+        win = {"window": meta["window"]} if meta.get("window") else {}
+        attn, lse = ops.attn_fwd(q, k, v, causal=True, kmask=meta["kmask"], need_lse=True, **win)
         attn2 = attn.view(rows, nh * hd)
         if fp8:
             x1 = ops.gemm_fp8(ops.fp8_quantize_act(attn2), train_fp8.weight_rows(o_w), residual=x2)
@@ -660,9 +662,12 @@ class DecoderLayerFn(torch.autograd.Function):
     def forward(ctx, meta, x, ln1, q_w, k_w, v_w, o_w, ln2, gate_w, up_w, down_w):
         # q_w/k_w/v_w and gate_w/up_w are the HF-named leaf parameters (for autograd bookkeeping); the GEMMs use the
         # fused views meta["qkv_w"] / meta["gu_w"] over the same storage (CBLlamaDecoderLayer._fused()).
+        return DecoderLayerFn._forward_saving(ctx, meta, x, ln1, meta["qkv_w"], o_w, ln2, meta["gu_w"], down_w)
+
+    @staticmethod
+    def _forward_saving(ctx, meta, x, ln1, qkv_w, o_w, ln2, gu_w, down_w):
         keep = not meta["recompute"]
         _await(*meta["params"])
-        qkv_w, gu_w = meta["qkv_w"], meta["gu_w"]
         out, saved = DecoderLayerFn._forward(meta, x, ln1, qkv_w, o_w, ln2, gu_w, down_w, keep)
         ctx.meta = meta
         if keep:
@@ -674,6 +679,20 @@ class DecoderLayerFn(torch.autograd.Function):
     @staticmethod
     @_ranged("decoder_layer.bwd")
     def backward(ctx, dout):
+        nh, nkv, hd = ctx.meta["nh"], ctx.meta["nkv"], ctx.meta["hd"]
+        dx, g_ln1, g_qkv, g_o, g_ln2, g_gu, g_down = DecoderLayerFn._backward(ctx, dout)
+        gq = gk = gv = gg = gup = None
+        if g_qkv is not None:  # no main_grad buffers: hand autograd the per-parameter slices of the fused gradient
+            gq, gk, gv = g_qkv[: nh * hd], g_qkv[nh * hd:(nh + nkv) * hd], g_qkv[(nh + nkv) * hd:]
+        if g_gu is not None:
+            I = g_gu.shape[0] // 2
+            gg, gup = g_gu[:I], g_gu[I:]
+        return None, dx, g_ln1, gq, gk, gv, g_o, g_ln2, gg, gup, g_down
+
+    @staticmethod
+    def _backward(ctx, dout):
+        """-> dx, then the gradients of ln1, the fused qkv weight, o, ln2, the fused gate|up weight and down (None where
+        they went to main_grad or the parameter is frozen)."""
         meta = ctx.meta
         sv = ctx.saved_tensors
         x, ln1, qkv_w, o_w, ln2, gu_w, down_w = sv[:7]
@@ -727,9 +746,10 @@ class DecoderLayerFn(torch.autograd.Function):
         q = qkv[:, : nh * hd].view(B, S, nh, hd)
         k = qkv[:, nh * hd:(nh + nkv) * hd].view(B, S, nkv, hd)
         v = qkv[:, (nh + nkv) * hd:].view(B, S, nkv, hd)
+        win = {"window": meta["window"]} if meta.get("window") else {}
         ops.attn_bwd(q, k, v, attn, dattn.view(B, S, nh, hd), lse, causal=True, kmask=meta["kmask"],
                      dq=dqkv[:, : nh * hd].view(B, S, nh, hd), dk=dqkv[:, nh * hd:(nh + nkv) * hd].view(B, S, nkv, hd),
-                     dv=dqkv[:, (nh + nkv) * hd:].view(B, S, nkv, hd))
+                     dv=dqkv[:, (nh + nkv) * hd:].view(B, S, nkv, hd), **win)
         ops.rope_(dqkv, meta["pos"], meta["cos"], meta["sin"], nh + nkv, hd, inverse=True)
         h = ops.rmsnorm_fwd(x2, ln1, meta["eps"], meta["hf_cast"])
         dh = dgrad(dqkv, qkv_w)
@@ -737,12 +757,25 @@ class DecoderLayerFn(torch.autograd.Function):
         del dqkv, h
         dx, dg1 = ops.rmsnorm_bwd(dh, x2, ln1, rstd1, dres=dx1)
         g_ln1 = vgrad(p_ln1, dg1)
-        gq = gk = gv = gg = gup = None
-        if g_qkv is not None:  # no main_grad buffers: hand autograd the per-parameter slices of the fused gradient
-            gq, gk, gv = g_qkv[: nh * hd], g_qkv[nh * hd:(nh + nkv) * hd], g_qkv[(nh + nkv) * hd:]
-        if g_gu is not None:
-            gg, gup = g_gu[:I], g_gu[I:]
-        return None, dx.view(B, S, H), g_ln1, gq, gk, gv, g_o, g_ln2, gg, gup, g_down
+        return dx.view(B, S, H), g_ln1, g_qkv, g_o, g_ln2, g_gu, g_down
+
+
+class FusedDecoderLayerFn(torch.autograd.Function):
+    _nvtx = "DecoderLayer"
+
+    """DecoderLayerFn for a layer whose fused weights are themselves the leaf parameters (Phi-3's qkv_proj and
+    gate_up_proj): x [B,S,H] -> x'; arguments ln1, qkv_w, o_w, ln2, gu_w, down_w, and the same meta, whose params hold
+    the six leaves (each with its own main_grad under TrainEngine)."""
+
+    @staticmethod
+    @_ranged("decoder_layer.fwd")
+    def forward(ctx, meta, x, ln1, qkv_w, o_w, ln2, gu_w, down_w):
+        return DecoderLayerFn._forward_saving(ctx, meta, x, ln1, qkv_w, o_w, ln2, gu_w, down_w)
+
+    @staticmethod
+    @_ranged("decoder_layer.bwd")
+    def backward(ctx, dout):
+        return (None, *DecoderLayerFn._backward(ctx, dout))
 
 
 # ------------------------------------------------------------------------------------------------------------------

@@ -288,10 +288,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 // ------------------------------------------------------------------------------------------------
 // delta[b, h, s] = sum_d dO[b,s,h,d] * O[b,s,h,d]   (fp32).  hd / 8 lanes (one 16-byte vector each) per (b, s, h), so a
 // warp covers 32 / (hd / 8) heads: with one warp per head only hd / 8 of the 32 lanes had work (2.2 TB/s).
+// PAD (hd 96, whose 12 lanes per head do not divide 32): 16 lanes per head, the last 4 idle.
+template <bool PAD>
 __global__ void attn_delta_kernel(const bf16* __restrict__ o, const bf16* __restrict__ d_o, float* __restrict__ delta,
                                   int B, int S, int nh, int hd, long long o_bs, long long o_ss, long long do_bs,
                                   long long do_ss) {
-  const int lph = hd >> 3;                       // lanes per head: 16 (hd 128) or 8 (hd 64)
+  const int lph = PAD ? 16 : hd >> 3;            // lanes per head: 16 (hd 96, 128) or 8 (hd 64)
   const int hpw = 32 / lph;                      // heads per warp
   const long long w = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -299,7 +301,7 @@ __global__ void attn_delta_kernel(const bf16* __restrict__ o, const bf16* __rest
   const long long idx = w * hpw + lane / lph;    // (b, s, h) handled by this lane group
   const int sub = lane % lph;
   float acc = 0.f;
-  if (idx < total) {
+  if (idx < total && (!PAD || sub * 8 < hd)) {
     const int h = (int)(idx % nh);
     const long long t = idx / nh;
     const int s = (int)(t % S);
@@ -330,11 +332,15 @@ struct AttnBwdParams {
   const uint8_t* kmask;
   int B, nh, nkv, Sq, Skv, hd, causal;
   float scale_log2, scale;
+  int window;               // sliding window (WIN kernels), the forward's rule: key slot j visible from query slot i
+                            // iff 0 <= i - j < window
 };
 
+// hd 96 computes on one and a half 64-column swizzle atoms, its tiles padded to two in shared memory (the TMA box past
+// column 96 zero-fills): hd 128's footprint
 template <int HDP>
 struct BwdCfg {
-  static constexpr int ATOMS = HDP / 64;
+  static constexpr int ATOMS = (HDP + 63) / 64;
   static constexpr int KTILE = ATOMS * 16384;  // [128 keys x hd]
   static constexpr int QTILE = ATOMS * 8192;   // [64 queries x hd]
   static constexpr int STAGES = 4;             // Q / dO ring; each stage also holds the tile's lse[64] and delta[64]
@@ -344,7 +350,10 @@ struct BwdCfg {
 // 384 threads: warpgroups 0-1 consume (dK and dV alone hold HDP fp32 per thread), warp 8 of warpgroup 2 produces.
 // Registers are allocated per 4 warps, so a 288-thread CTA would cap every thread at 168; setmaxnreg moves the
 // producer warpgroup's share to the consumers instead (128 x 24 + 256 x 240 <= 64 K).
-template <int HDP>
+// WIN: causal sliding window (p.window > 0).  The query tiles stop after the last query whose window reaches the CTA's
+// last key; a warpgroup skips a tile whose queries all lie past the window of its 64 keys, and tiles on the window's
+// edge take the per-element path.  WIN = false compiles to the plain kernel.
+template <int HDP, bool WIN>
 __global__ void __launch_bounds__(384, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, AttnBwdParams p) {
@@ -376,7 +385,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const int first_q = k0 - coff;
     i_begin = first_q > 0 ? first_q / 64 : 0;
   }
-  const int n_i = q_tiles > i_begin ? q_tiles - i_begin : 0;
+  int i_end = q_tiles;
+  if (WIN) {  // the last query slot that sees key k0 + 127 is k0 + 127 + window - 1
+    const int last_q = k0 + 127 + p.window - 1 - coff;
+    i_end = last_q < 0 ? 0 : min(q_tiles, last_q / 64 + 1);
+  }
+  const int n_i = i_end > i_begin ? i_end - i_begin : 0;
   const int n_iter = n_i * G;
 
   if (warp == 8 && lane == 0) {
@@ -457,6 +471,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const int qi0 = (i_begin + it % n_i) * 64;
     const uint32_t qb = sQ + st * Cfg::QTILE, dob = sdO + st * Cfg::QTILE;
     mbar_wait(qd_full(st), ph);
+    if (WIN && qi0 + coff > k0 + wg * 64 + 63 + p.window - 1) {
+      // every query of the tile lies past the window of all 64 keys of this warpgroup: release the stage, no work
+      if (lane == 0) mbar_arrive(qd_empty(st));
+      if (++st == STAGES) { st = 0; ph ^= 1u; }
+      continue;
+    }
     float sT[32], dpT[32];
     wgmma_fence();
 #pragma unroll
@@ -474,7 +494,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     wgmma_commit();
     // every (key, query) pair of the tile is visible to this warp: all 64 queries exist, the warp's 16 keys are valid
     // and none lies past the diagonal of the tile's first query
-    const bool full = warp_keys_ok && qi0 + 64 <= p.Sq && (!p.causal || wk0 + 15 <= qi0 + coff);
+    bool full = warp_keys_ok && qi0 + 64 <= p.Sq && (!p.causal || wk0 + 15 <= qi0 + coff);
+    if (WIN) full = full && qi0 + 63 + coff - wk0 < p.window;  // the tile's last query still sees the warp's first key
     const float* ld = ld_stage + st * 128;
     wgmma_wait<0>();
     reg_fence(sT);
@@ -495,7 +516,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
             const int e = 2 * r + c;
             bool vis = true;
             if (!decltype(full_tile)::value)
-              vis = qi0 + qc < p.Sq && key_ok[r] && (!p.causal || k0 + kr + 8 * r <= qi0 + qc + coff);
+              vis = qi0 + qc < p.Sq && key_ok[r] && (!p.causal || k0 + kr + 8 * r <= qi0 + qc + coff) &&
+                    (!WIN || qi0 + qc + coff - (k0 + kr + 8 * r) < p.window);
             const float pe = vis ? fast_exp2(fmaf(sT[4 * jj + e], p.scale_log2, -L)) : 0.f;
             pv[e] = pe;
             dsv[e] = pe * (dpT[4 * jj + e] - D);
@@ -545,14 +567,17 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
 template <int HDP>
 struct DqCfg {
-  static constexpr int ATOMS = HDP / 64;
+  static constexpr int ATOMS = (HDP + 63) / 64;
   static constexpr int QTILE = ATOMS * 16384;  // [128 queries x hd]
   static constexpr int KTILE = ATOMS * 8192;   // [64 keys x hd]
   static constexpr int STAGES = 4;
   static constexpr int SMEM = 2 * QTILE + 2 * STAGES * KTILE + 1024 + 256;
 };
 
-template <int HDP>
+// WIN: causal sliding window (p.window > 0).  The producer starts at the first key tile inside the window of the CTA's
+// first query; a warpgroup skips a tile that lies wholly before the window of all its 64 rows, and tiles on the
+// window's edge take the per-element path.  WIN = false compiles to the plain kernel.
+template <int HDP, bool WIN>
 __global__ void __launch_bounds__(288, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, AttnBwdParams p) {
@@ -580,6 +605,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int kv_tiles_all = (p.Skv + 63) / 64;
   int n_tiles = kv_tiles_all;
   if (p.causal) n_tiles = max(1, min(kv_tiles_all, (q0 + 127 + coff) / 64 + 1));
+  int j_lo = 0;
+  if (WIN) j_lo = min(n_tiles - 1, max(0, q0 + coff - p.window + 1) / 64);
 
   if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmQ);
@@ -606,7 +633,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       }
       int st = 0;
       uint32_t ph = 0;
-      for (int j = 0; j < n_tiles; ++j) {
+      for (int j = j_lo; j < n_tiles; ++j) {
         mbar_wait(kv_empty(st), ph ^ 1u);
         mbar_arrive_expect_tx(kv_full(st), 2 * Cfg::KTILE);
 #pragma unroll
@@ -643,9 +670,15 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   mbar_wait(q_full, 0);
   int st = 0;
   uint32_t ph = 0;
-  for (int j = 0; j < n_tiles; ++j) {
+  for (int j = j_lo; j < n_tiles; ++j) {
     const int k0 = j * 64;
     mbar_wait(kv_full(st), ph);
+    if (WIN && k0 + 63 < q0 + wg * 64 + coff - p.window + 1) {
+      // before the window of all 64 rows of this warpgroup: release the stage, no work
+      if (wg_leader) mbar_arrive(kv_empty(st));
+      if (++st == STAGES) { st = 0; ph ^= 1u; }
+      continue;
+    }
     const uint32_t kb = sK + st * Cfg::KTILE, vb = sV + st * Cfg::KTILE;
     float s[32], dp[32];
     wgmma_fence();
@@ -665,6 +698,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     // every (query, key) pair of the tile is visible to this warp: the 64 keys lie inside Skv, at or before the
     // diagonal of the warp's first query, and are all valid; the warp's 16 queries exist
     bool full = k0 + 64 <= p.Skv && wq0 + 16 <= p.Sq && (!p.causal || k0 + 63 <= wq0 + coff);
+    if (WIN) full = full && wq0 + 15 + coff - k0 < p.window;  // the warp's last query still sees the tile's first key
     if (full && km) full = keys_all_valid<64>(km, k0);
     wgmma_wait<0>();
     reg_fence(s);
@@ -680,7 +714,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           const int r = e >> 1, key = k0 + 8 * jj + cq + (e & 1);
           bool vis = true;
           if (!decltype(full_tile)::value)
-            vis = qi[r] < p.Sq && key < p.Skv && (!p.causal || key <= qi[r] + coff) && (!km || km[key]);
+            vis = qi[r] < p.Sq && key < p.Skv && (!p.causal || key <= qi[r] + coff) && (!km || km[key]) &&
+                  (!WIN || qi[r] + coff - key < p.window);
           const float pe = vis ? fast_exp2(fmaf(s[4 * jj + e], p.scale_log2, -L[r])) : 0.f;
           dsv[e] = pe * (dp[4 * jj + e] - D[r]);
         }
@@ -806,11 +841,11 @@ int attn_fwd_launch(const void* q, const void* k, const void* v, void* o, float*
   return launch_fwd<128, false>(tq, tk, tv, p, st);
 }
 
-template <int HDP>
+template <int HDP, bool WIN>
 static int launch_bwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tdo,
                       const AttnBwdParams& p, cudaStream_t st) {
   using Cfg = BwdCfg<HDP>;
-  auto kern = attn_bwd_kernel<HDP>;
+  auto kern = attn_bwd_kernel<HDP, WIN>;
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
@@ -822,11 +857,11 @@ static int launch_bwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtens
   return CB_OK;
 }
 
-template <int HDP>
+template <int HDP, bool WIN>
 static int launch_bwd_dq(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tdo,
                          const AttnBwdParams& p, cudaStream_t st) {
   using Cfg = DqCfg<HDP>;
-  auto kern = attn_bwd_dq_kernel<HDP>;
+  auto kern = attn_bwd_dq_kernel<HDP, WIN>;
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
@@ -838,22 +873,33 @@ static int launch_bwd_dq(const CUtensorMap& tq, const CUtensorMap& tk, const CUt
   return CB_OK;
 }
 
+// dK / dV from 64-query Q / dO tiles against 128-key K / V tiles, then dQ from 128-query tiles against 64-key tiles
+template <int HDP, bool WIN>
+static int launch_bwd_both(const CUtensorMap (&t)[4], const CUtensorMap (&tdq)[4], const AttnBwdParams& p,
+                           cudaStream_t st) {
+  if (int rc = launch_bwd<HDP, WIN>(t[0], t[1], t[2], t[3], p, st)) return rc;
+  return launch_bwd_dq<HDP, WIN>(tdq[0], tdq[1], tdq[2], tdq[3], p, st);
+}
+
 int attn_bwd_launch(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                     float* delta, void* dq, void* dk, void* dv, const void* kmask, int B, int nh, int nkv,
                     int Sq, int Skv, int hd, long long q_bs, long long q_ss, long long k_bs, long long k_ss,
                     long long v_bs, long long v_ss, long long o_bs, long long o_ss, long long do_bs, long long do_ss,
                     long long dq_bs, long long dq_ss, long long dk_bs, long long dk_ss, long long dv_bs,
-                    long long dv_ss, float scale, int causal, cudaStream_t st) {
+                    long long dv_ss, float scale, int causal, int window, cudaStream_t st) {
   CB_CHECK_ARG(B > 0 && nh > 0 && nkv > 0 && Sq > 0 && Skv > 0, "attention bwd: empty problem");
+  CB_CHECK_ARG(window >= 0 && (window == 0 || causal), "attention bwd: window=%d needs causal attention (0 = none)",
+               window);
   CB_CHECK_ARG(nh % nkv == 0, "attention bwd: nh=%d not a multiple of nkv=%d", nh, nkv);
-  CB_CHECK_ARG(hd == 64 || hd == 128, "attention bwd: head_dim=%d unsupported (64 or 128)", hd);
+  CB_CHECK_ARG(hd == 64 || hd == 96 || hd == 128, "attention bwd: head_dim=%d unsupported (64, 96 or 128)", hd);
   CB_CHECK_ARG(lse && delta && dq && dk && dv, "attention bwd: lse / delta / dq / dk / dv buffers are required");
   CB_CHECK_ARG(!(reinterpret_cast<uintptr_t>(dq) & 3u) && dq_bs % 2 == 0 && dq_ss % 2 == 0,
                "attention bwd: dq must be 4-byte aligned with even strides");
   {
     const long long warps = ((long long)B * Sq * nh + (256 / hd) - 1) / (256 / hd);   // 32 / (hd / 8) heads per warp
-    attn_delta_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>((const bf16*)o, (const bf16*)d_o, delta, B,
-                                                                           Sq, nh, hd, o_bs, o_ss, do_bs, do_ss);
+    auto kern = hd == 96 ? attn_delta_kernel<true> : attn_delta_kernel<false>;       // hd 96: 2 heads per warp
+    kern<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>((const bf16*)o, (const bf16*)d_o, delta, B, Sq, nh, hd,
+                                                              o_bs, o_ss, do_bs, do_ss);
     CB_CUDA_LAUNCH_CHECK("attn_delta");
   }
   CUtensorMap tq, tk, tv, tdo;
@@ -868,18 +914,23 @@ int attn_bwd_launch(const void* q, const void* k, const void* v, const void* o, 
   p.lse = lse; p.delta = delta; p.kmask = (const uint8_t*)kmask;
   p.B = B; p.nh = nh; p.nkv = nkv; p.Sq = Sq; p.Skv = Skv; p.hd = hd; p.causal = causal;
   p.scale_log2 = scale * LOG2E; p.scale = scale;
+  p.window = window;
   // the dQ kernel streams 64-key K / V tiles against 128-query Q / dO tiles
-  CUtensorMap tq128, tk64, tv64, tdo128;
-  if ((rc = make_tmap_bf16_4d(&tq128, q, hd, nh, Sq, B, hd, q_ss, q_bs, 128))) return rc;
-  if ((rc = make_tmap_bf16_4d(&tk64, k, hd, nkv, Skv, B, hd, k_ss, k_bs, 64))) return rc;
-  if ((rc = make_tmap_bf16_4d(&tv64, v, hd, nkv, Skv, B, hd, v_ss, v_bs, 64))) return rc;
-  if ((rc = make_tmap_bf16_4d(&tdo128, d_o, hd, nh, Sq, B, hd, do_ss, do_bs, 128))) return rc;
-  if (hd == 64) {
-    if ((rc = launch_bwd<64>(tq, tk, tv, tdo, p, st))) return rc;
-    return launch_bwd_dq<64>(tq128, tk64, tv64, tdo128, p, st);
+  CUtensorMap tdq[4];
+  if ((rc = make_tmap_bf16_4d(&tdq[0], q, hd, nh, Sq, B, hd, q_ss, q_bs, 128))) return rc;
+  if ((rc = make_tmap_bf16_4d(&tdq[1], k, hd, nkv, Skv, B, hd, k_ss, k_bs, 64))) return rc;
+  if ((rc = make_tmap_bf16_4d(&tdq[2], v, hd, nkv, Skv, B, hd, v_ss, v_bs, 64))) return rc;
+  if ((rc = make_tmap_bf16_4d(&tdq[3], d_o, hd, nh, Sq, B, hd, do_ss, do_bs, 128))) return rc;
+  const CUtensorMap t[4] = {tq, tk, tv, tdo};
+  // the largest query-key distance is Skv - 1: a window of Skv or more hides nothing and takes the plain kernels
+  if (window > 0 && window < Skv) {
+    if (hd == 64) return launch_bwd_both<64, true>(t, tdq, p, st);
+    if (hd == 96) return launch_bwd_both<96, true>(t, tdq, p, st);
+    return launch_bwd_both<128, true>(t, tdq, p, st);
   }
-  if ((rc = launch_bwd<128>(tq, tk, tv, tdo, p, st))) return rc;
-  return launch_bwd_dq<128>(tq128, tk64, tv64, tdo128, p, st);
+  if (hd == 64) return launch_bwd_both<64, false>(t, tdq, p, st);
+  if (hd == 96) return launch_bwd_both<96, false>(t, tdq, p, st);
+  return launch_bwd_both<128, false>(t, tdq, p, st);
 }
 
 }  // namespace cb

@@ -80,9 +80,8 @@ class TrainEngine:
                  background_optimizer: bool = False, collective: str = "nccl", offload_optimizer: bool = False):
         if zero_stage not in (0, 2):
             raise ValueError("zero_stage must be 0 or 2")
-        if getattr(getattr(model, "config", None), "model_type", None) == "cambrian_phi3":
-            from .model.language_model.cambrian_phi3 import TRAINING_REFUSAL
-            raise NotImplementedError(f"TrainEngine: {TRAINING_REFUSAL}")
+        if hasattr(model, "check_trainable"):   # a model that trains only in some configurations refuses the others
+            model.check_trainable()
         from .quant import quantized_format
         fmt = quantized_format(model)
         if fmt is not None:

@@ -187,14 +187,19 @@ class CBLlamaDecoderLayer(nn.Module):
         fp8 = bool(rt.get("fp8", False))
         if fp8:
             train_fp8.check_widths(x.shape[-1], gu_w.shape[0] // 2, qkv_w.shape[0])
-        meta = dict(nh=self.nh, nkv=self.nkv, hd=self.hd, eps=self.input_layernorm.variance_epsilon,
-                    hf_cast=rt["hf_cast"], cos=rt["cos"], sin=rt["sin"], pos=rt["pos"], kmask=rt["kmask"],
-                    recompute=rt["recompute"], fp8=fp8, qkv_w=qkv_w, gu_w=gu_w,
-                    params=(self.input_layernorm.weight, g_qkv, a.o_proj.weight, self.post_attention_layernorm.weight,
-                            g_gu, m.down_proj.weight))
+        meta = self._train_meta(rt, g_qkv, g_gu, fp8=fp8, qkv_w=qkv_w, gu_w=gu_w)
         return DecoderLayerFn.apply(meta, x, self.input_layernorm.weight, a.q_proj.weight, a.k_proj.weight,
                                     a.v_proj.weight, a.o_proj.weight, self.post_attention_layernorm.weight,
                                     m.gate_proj.weight, m.up_proj.weight, m.down_proj.weight)
+
+    def _train_meta(self, rt, qkv_grad, gu_grad, **extra):
+        """DecoderLayerFn's meta; qkv_grad / gu_grad: what receives the fused weights' gradients (see `params`)."""
+        a, m = self.self_attn, self.mlp
+        return dict(nh=self.nh, nkv=self.nkv, hd=self.hd, eps=self.input_layernorm.variance_epsilon,
+                    hf_cast=rt["hf_cast"], cos=rt["cos"], sin=rt["sin"], pos=rt["pos"], kmask=rt["kmask"],
+                    recompute=rt["recompute"], **extra,
+                    params=(self.input_layernorm.weight, qkv_grad, a.o_proj.weight, self.post_attention_layernorm.weight,
+                            gu_grad, m.down_proj.weight))
 
     @torch.no_grad()
     def infer(self, x, rt, cache):

@@ -1,11 +1,11 @@
 """CambrianPhi3ForCausalLM — H100-native mirror of the reference's `cambrian/model/language_model/cambrian_phi3.py`
-(Cambrian-Phi3-3B), for inference.
+(Cambrian-Phi3-3B), for inference and training.
 
 Phi-3-mini is the LLaMA decoder with three differences, and this file adds only those:
   * fused projections under Phi-3's state-dict keys: `self_attn.qkv_proj` ([q | k | v] rows) and `mlp.gate_up_proj`
     ([gate | up] rows) — exactly the layouts `fuse_rows` builds for LLaMA, so they feed the same GEMM / SwiGLU kernels
     as they are, without copies;
-  * head dim 96 (hidden 3072 / 32 heads), which the flash-attention forward instantiates;
+  * head dim 96 (hidden 3072 / 32 heads), which the flash-attention forward and backward instantiate;
   * a causal sliding window (`config.sliding_window`, 2047 in the released checkpoints).  The reference loads the model
     with `use_flash_attention_2=False`, so its mask is transformers' `_prepare_4d_causal_attention_mask(...,
     sliding_window=W)` as of the transformers 4.37 it pins: key slot j is visible from query slot i iff 0 <= i - j < W,
@@ -14,12 +14,17 @@ Phi-3-mini is the LLaMA decoder with three differences, and this file adds only 
 
 Everything else is shared with CambrianLlamaForCausalLM: the decoder layer's `infer` (the layer hands it its fused
 weights through `_fused()` and its window through `window`), `KVCache`, `generate()` and its CUDA-graph decode loop, and
-the multimodal front end of cambrian_arch.py (towers, SVA connector, in-LLM SVA sites).
+the multimodal front end of cambrian_arch.py (towers, SVA connector, in-LLM SVA sites).  In training each layer runs
+autograd.FusedDecoderLayerFn — DecoderLayerFn's forward and backward with the fused `qkv_proj` / `gate_up_proj` weights
+as the leaf parameters (each with its own `main_grad` under TrainEngine) and the window passed to both attention calls,
+recompute included.  The reference trains Phi-3 with eager attention (`_supports_sdpa = False`) under the same mask, its
+RMSNorm in fp32 (`hf_cast=False` in training, as for LLaMA).
 
-Not supported, each refused with an exception that names it: training (the head-dim-96 flash-attention backward and
-sliding-window training do not exist), NF4 / LLM.int8 / FP8 weights (the quantisers address the LLaMA projections by
-name), the FP8 KV cache (its decode kernel takes head dims 64 and 128), Zero3Inference, and `rope_scaling` (the 128k
-`su` / `yarn` variants).
+Not supported, each refused with an exception that names it: training on parameters that are not all CUDA bf16 (the
+attention backward has no CPU path), non-zero `attention_dropout` / `resid_pdrop` / `embd_pdrop` (dropout is not
+implemented; Phi-3-mini's are 0), `fp8_training`, NF4 / LLM.int8 / FP8 weights (the quantisers address the LLaMA
+projections by name), the FP8 KV cache (its decode kernel takes head dims 64 and 128), Zero3Inference, and
+`rope_scaling` (the 128k `su` / `yarn` variants).
 """
 from __future__ import annotations
 
@@ -27,11 +32,11 @@ import torch
 import torch.nn as nn
 from transformers import AutoConfig, AutoModelForCausalLM, PretrainedConfig
 
+from ...autograd import FusedDecoderLayerFn
 from .cambrian_llama import (CambrianLlamaForCausalLM, CambrianLlamaModel, CambrianPreTrainedModel, CBLlamaDecoderLayer,
                              CBRMSNorm)
 
-TRAINING_REFUSAL = ("Cambrian-Phi3 is inference-only here: training needs the head-dim-96 flash-attention backward and "
-                    "sliding-window attention backward, which do not exist; run it under torch.no_grad()")
+DROPOUT_FIELDS = ("attention_dropout", "resid_pdrop", "embd_pdrop")
 
 
 class CambrianPhi3Config(PretrainedConfig):
@@ -78,6 +83,27 @@ def check_supported(config):
         raise NotImplementedError(f"Cambrian-Phi3 with hidden_act={config.hidden_act!r}: the SwiGLU kernel is SiLU only")
 
 
+def require_cuda_bf16(model):
+    """Training runs the CUDA kernels only: refuse parameters that are not all CUDA bf16."""
+    if any(p.device.type != "cuda" or p.dtype != torch.bfloat16 for p in model.parameters()):
+        raise NotImplementedError("Cambrian-Phi3 trains in bf16 on CUDA only: its head-dim-96 / sliding-window "
+                                  "flash-attention backward has no CPU path; move the model to CUDA in bf16, or run "
+                                  "it under torch.no_grad()")
+
+
+def check_trainable(model):
+    """Refuse the training configurations that are not implemented, before the first kernel runs."""
+    cfg = model.config
+    for name in DROPOUT_FIELDS:
+        if getattr(cfg, name, 0.0):
+            raise NotImplementedError(f"training Cambrian-Phi3 with {name}={getattr(cfg, name)} is not supported: "
+                                      "dropout is not implemented (Phi-3-mini's dropouts are 0)")
+    if getattr(cfg, "fp8_training", False):
+        raise NotImplementedError("Cambrian-Phi3 with fp8_training is not supported: FP8 training is validated for "
+                                  "the LLaMA decoder only")
+    require_cuda_bf16(model)
+
+
 class CBPhi3Attention(nn.Module):
     def __init__(self, config):
         super().__init__()
@@ -95,7 +121,7 @@ class CBPhi3MLP(nn.Module):
 
 
 class CBPhi3DecoderLayer(CBLlamaDecoderLayer):
-    """Phi3DecoderLayer under its state-dict keys; runs CBLlamaDecoderLayer.infer (dropouts are identities at inference)."""
+    """Phi3DecoderLayer under its state-dict keys: FusedDecoderLayerFn under grad, CBLlamaDecoderLayer.infer without."""
 
     def __init__(self, config, layer_idx):
         nn.Module.__init__(self)
@@ -114,9 +140,13 @@ class CBPhi3DecoderLayer(CBLlamaDecoderLayer):
         return self.self_attn.qkv_proj.weight, self.mlp.gate_up_proj.weight, None, None
 
     def forward(self, x, rt):
-        if torch.is_grad_enabled():
-            raise NotImplementedError(TRAINING_REFUSAL)
-        return self.infer(x, rt, None)
+        if not torch.is_grad_enabled():
+            return self.infer(x, rt, None)
+        a, m = self.self_attn, self.mlp
+        ln1, ln2 = self.input_layernorm.weight, self.post_attention_layernorm.weight
+        qkv_w, gu_w = a.qkv_proj.weight, m.gate_up_proj.weight
+        meta = self._train_meta(rt, qkv_w, gu_w, window=self.window)
+        return FusedDecoderLayerFn.apply(meta, x, ln1, qkv_w, a.o_proj.weight, ln2, gu_w, m.down_proj.weight)
 
 
 class CambrianPhi3Model(CambrianLlamaModel):
@@ -139,10 +169,14 @@ class CambrianPhi3ForCausalLM(CambrianLlamaForCausalLM):
     def attention_window(self) -> int:
         return int(getattr(self.config, "sliding_window", None) or 0)
 
+    def check_trainable(self):
+        """TrainEngine's and the grad-mode forward's check: see `check_trainable`."""
+        check_trainable(self)
+
     def forward(self, *args, **kwargs):
-        """cambrian_phi3.py's forward (the Phi3ForCausalLM outputs: loss, logits, past_key_values), inference only."""
+        """cambrian_phi3.py's forward (the Phi3ForCausalLM outputs: loss, logits, past_key_values)."""
         if torch.is_grad_enabled():
-            raise NotImplementedError(TRAINING_REFUSAL)
+            check_trainable(self)
         return super().forward(*args, **kwargs)
 
     @torch.no_grad()

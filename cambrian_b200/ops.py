@@ -319,8 +319,10 @@ def attn_fwd(q, k, v, *, causal: bool, kmask=None, scale: float | None = None, n
     return (o, lse) if need_lse else o
 
 
-def attn_bwd(q, k, v, o, do, lse, *, causal: bool, kmask=None, scale: float | None = None, dq=None, dk=None, dv=None):
-    """Returns dq [B,Sq,nh,hd], dk, dv [B,Skv,nkv,hd] (bf16).  dq/dk/dv may be preallocated (strided views ok)."""
+def attn_bwd(q, k, v, o, do, lse, *, causal: bool, kmask=None, scale: float | None = None, dq=None, dk=None, dv=None,
+             window: int = 0):
+    """Returns dq [B,Sq,nh,hd], dk, dv [B,Skv,nkv,hd] (bf16).  dq/dk/dv may be preallocated (strided views ok).
+    window: the sliding window the forward ran with (see attn_fwd); a query row that sees no key gets dq = 0."""
     _require_cuda_bf16(q, k, v, o, do)
     B, Sq, nh, hd = q.shape
     Skv, nkv = k.shape[1], k.shape[2]
@@ -342,6 +344,13 @@ def attn_bwd(q, k, v, o, do, lse, *, causal: bool, kmask=None, scale: float | No
     if kmask is not None:
         kmask = kmask.contiguous()
         kmask = kmask.view(torch.uint8) if kmask.dtype == torch.bool else kmask.to(torch.uint8)
+    if window:
+        rc = _lib.load().cb_attn_bwd_window(ptr(q), ptr(k), ptr(v), ptr(o), ptr(do), ptr(lse), ptr(delta), ptr(dq),
+                                            ptr(dk), ptr(dv), ptr(kmask), B, nh, nkv, Sq, Skv, hd, qb, qs, kb, ks, vb,
+                                            vs_, ob, os_, dob, dos, dqb, dqs, dkb, dks, dvb, dvs, float(scale),
+                                            int(causal), int(window), stream())
+        check(rc, "cb_attn_bwd_window")
+        return dq, dk, dv
     rc = _lib.load().cb_attn_bwd(ptr(q), ptr(k), ptr(v), ptr(o), ptr(do), ptr(lse), ptr(delta), ptr(dq), ptr(dk),
                                  ptr(dv), ptr(kmask), B, nh, nkv, Sq, Skv, hd, qb, qs, kb, ks, vb, vs_, ob, os_, dob, dos,
                                  dqb, dqs, dkb, dks, dvb, dvs, float(scale), int(causal), stream())

@@ -103,7 +103,7 @@ int64_t cb_norm_bwd_workspace_floats(int64_t rows, int C);
  * causal: key k visible to query i iff k <= i + (Skv - Sq).  lse [B, nh, Sq] fp32 (log2 domain) may be NULL.
  * Replaces torch SDPA inside HF CLIPAttention / Dinov2SelfAttention / timm Attention (clip_encoder.py:104,
  * dino_encoder.py:159, siglip_encoder.py:97) and HF LlamaSdpaAttention with the 4-D causal+padding mask of
- * cambrian_llama.py:123-128.  head_dim: any multiple of 8 up to 128 (fwd); 64 or 128 (bwd). */
+ * cambrian_llama.py:123-128.  head_dim: any multiple of 8 up to 128 (fwd); 64, 96 or 128 (bwd). */
 int cb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, const void* kmask, int B, int nh,
                 int nkv, int Sq, int Skv, int hd, int64_t q_bs, int64_t q_ss, int64_t k_bs, int64_t k_ss,
                 int64_t v_bs, int64_t v_ss, int64_t o_bs, int64_t o_ss, float scale, int causal, void* stream);
@@ -121,6 +121,16 @@ int cb_attn_bwd(const void* q, const void* k, const void* v, const void* o, cons
                 int Skv, int hd, int64_t q_bs, int64_t q_ss, int64_t k_bs, int64_t k_ss, int64_t v_bs, int64_t v_ss,
                 int64_t o_bs, int64_t o_ss, int64_t do_bs, int64_t do_ss, int64_t dq_bs, int64_t dq_ss,
                 int64_t dk_bs, int64_t dk_ss, int64_t dv_bs, int64_t dv_ss, float scale, int causal, void* stream);
+/* cb_attn_bwd with the causal sliding window of cb_attn_fwd_window (pass the same window and the lse it wrote): query
+ * tiles past the window of a whole warpgroup's keys, and key tiles before the window of a whole warpgroup's queries,
+ * are skipped.  window = 0 means none and is cb_attn_bwd exactly; window > 0 needs causal = 1.  A query row that sees no
+ * key (lse = +inf) gets dq = 0. */
+int cb_attn_bwd_window(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                       float* delta, void* dq, void* dk, void* dv, const void* kmask, int B, int nh, int nkv, int Sq,
+                       int Skv, int hd, int64_t q_bs, int64_t q_ss, int64_t k_bs, int64_t k_ss, int64_t v_bs,
+                       int64_t v_ss, int64_t o_bs, int64_t o_ss, int64_t do_bs, int64_t do_ss, int64_t dq_bs,
+                       int64_t dq_ss, int64_t dk_bs, int64_t dk_ss, int64_t dv_bs, int64_t dv_ss, float scale,
+                       int causal, int window, void* stream);
 
 /* ---- elementwise / gather / reduction kernels (HBM-bound) -------------------------------------- */
 /* y = act(x), dx = dy * act'(x); n elements (n % 8 == 0).  nn.GELU of vision_sampler.py:241, cambrian_arch.py:49,56 */
