@@ -425,8 +425,9 @@ def embed_splice_bwd(dout, ids, img_start, d_embed, q_side: int, has_img: bool):
 
 
 def embed_grad_sorted(dout, ids, img_start, d_embed, q_side: int):
-    """Deterministic embedding-row gradient: d_embed[id] = sum over the text positions holding `id` of dout rows, summed in
-    position order (d_embed must be zero on entry).  The sort of 8 K token ids is device-side index plumbing (torch)."""
+    """Deterministic embedding-row gradient: d_embed[id] += sum over the text positions holding `id` of dout rows, summed in
+    position order (ids outside [0, vocab) add to row 0, the row embed_splice reads for them; rows of ids that do not occur
+    are not touched).  The sort of 8 K token ids is device-side index plumbing (torch)."""
     B, S, H = dout.shape
     vocab = d_embed.shape[0]
     keys = ids.reshape(B, S).clamp(min=0)

@@ -52,22 +52,23 @@ def f32_to_bf16(src, dst, scale=1.0, cols=None, out_ld=None):
     return dst
 
 
-def _window_pos(pos, rows, side, r):
-    """pos_embed row added to each latent: natural layout (row = (b, y, x) of a side x side grid) -> window position
-    (y % r) * r + (x % r); window-rearranged layout (side == 0) -> row % r^2."""
+def _norm_input(x, pos, side, r):
+    """x [rows, C] in fp32, plus the pos_embed row of each latent's window position rounded to bf16 (the kernels fuse the
+    bf16 add `latents + pos_embed` into the load): natural layout (row = (b, y, x) of a side x side grid) -> window
+    position (y % r) * r + (x % r); window-rearranged layout (side == 0) -> row % r^2."""
     if pos is None:
-        return 0
-    idx = torch.arange(rows)
+        return x.float()
+    idx = torch.arange(x.shape[0])
     if side == 0:
         w = idx % (r * r)
     else:
         w = ((idx // side) % side % r) * r + (idx % side) % r
-    return pos.float()[w]
+    return (x.float() + pos.float()[w]).to(torch.bfloat16).float()
 
 
 def layernorm_fwd(x, gamma, beta, eps=1e-5, pos=None, side=0, r=0, save_stats=False, out=None):
     C = x.shape[-1]
-    xp = x.reshape(-1, C).float() + _window_pos(pos, x.numel() // C, side, r)
+    xp = _norm_input(x.reshape(-1, C), pos, side, r)
     mean, var = xp.mean(-1), xp.var(-1, unbiased=False)
     rstd = torch.rsqrt(var + eps)
     y = ((xp - mean[:, None]) * rstd[:, None] * gamma.float() + (beta.float() if beta is not None else 0)).to(torch.bfloat16)
@@ -81,7 +82,7 @@ def layernorm_fwd(x, gamma, beta, eps=1e-5, pos=None, side=0, r=0, save_stats=Fa
 def layernorm_bwd(dy, x, gamma, mean, rstd, pos=None, side=0, r=0, has_beta=True, dres=None):
     C = x.shape[-1]
     dy2 = dy.reshape(-1, C).float()
-    xp = x.reshape(-1, C).float() + _window_pos(pos, x.numel() // C, side, r)
+    xp = _norm_input(x.reshape(-1, C), pos, side, r)
     xh = (xp - mean[:, None]) * rstd[:, None]
     g = dy2 * gamma.float()
     dx = rstd[:, None] * (g - g.mean(-1, keepdim=True) - xh * (g * xh).mean(-1, keepdim=True))
@@ -155,9 +156,18 @@ def tower_combine_bwd(logits, aggs, dout):
     return [(w[:, t:t + 1] * d).to(torch.bfloat16) for t in range(T)], dl.to(torch.bfloat16)
 
 
+def _store(y, out, accumulate):
+    """the kernels' epilogue: round y (+ out when accumulating) once into `out`, or return a fresh tensor."""
+    if out is None:
+        return y
+    out.copy_(y + out.float() if accumulate else y)
+    return out
+
+
 def pos_grad(dx, B, side, r, out=None, accumulate=False):
     C = dx.shape[-1]
-    return dx.float().reshape(B, side // r, r, side // r, r, C).sum((0, 1, 3)).reshape(r * r, C).to(torch.bfloat16)
+    y = dx.float().reshape(B, side // r, r, side // r, r, C).sum((0, 1, 3)).reshape(r * r, C)
+    return _store(y, out, accumulate) if out is not None else y.to(torch.bfloat16)
 
 
 def bilinear(x, h, w, th, tw, *, in_bs=None, out=None, out_ld=None, out_col0=0):
@@ -178,12 +188,15 @@ def bilinear_bwd(dout, h, w, th, tw):
 
 def group_colsum(x, groups, scale=1.0, out=None, accumulate=False, fp32=False):
     y = x.float().reshape(groups, -1, x.shape[-1]).sum(1) * scale
+    if out is not None:
+        return _store(y, out, accumulate)
     return y if fp32 else y.to(torch.bfloat16)
 
 
 def group_broadcast(dmean, rows_per_group, scale, out=None, accumulate=False):
     G, C = dmean.shape
-    return (dmean.float() * scale)[:, None, :].expand(G, rows_per_group, C).reshape(G * rows_per_group, C).to(torch.bfloat16)
+    y = (dmean.float() * scale)[:, None, :].expand(G, rows_per_group, C).reshape(G * rows_per_group, C)
+    return _store(y, out, accumulate) if out is not None else y.to(torch.bfloat16)
 
 
 def add_(dst, src):
@@ -193,7 +206,9 @@ def add_(dst, src):
 
 def adamw(p32, m, v, g16, p16, lr, beta1, beta2, eps, wd, step, grad_scale=1.0, clip_coef=None, background=False):
     """adamw_kernel (elementwise.cu): torch.optim.AdamW arithmetic on fp32 master / moments, bf16 gradients in, bf16 copy out."""
-    gs = float(clip_coef[0]) if clip_coef is not None else grad_scale
+    f32 = lambda x: float(torch.tensor(x, dtype=torch.float32))     # the kernel's hyper-parameters are fp32
+    lr, beta1, beta2, eps, wd = map(f32, (lr, beta1, beta2, eps, wd))
+    gs = float(clip_coef[0]) if clip_coef is not None else f32(grad_scale)
     g = g16.float() * gs
     bc1, bc2 = 1.0 - beta1 ** step, 1.0 - beta2 ** step
     p32.mul_(1.0 - lr * wd)
