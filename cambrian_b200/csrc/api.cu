@@ -86,6 +86,10 @@ int adamw_launch(float*, float*, float*, const void*, void*, long long, float, f
                  const float*, int, cudaStream_t);
 int adamw_host_launch(float*, float*, float*, const void*, void*, long long, float, float, float, float, float, int, float,
                       const float*, int, cudaStream_t);
+int adamw8_launch(float*, void*, void*, float*, float*, const void*, void*, long long, float, float, float, float, float, int,
+                  float, const float*, int, cudaStream_t);
+int adamw8_host_launch(float*, void*, void*, float*, float*, const void*, void*, long long, float, float, float, float, float,
+                       int, float, const float*, int, cudaStream_t);
 int sumsq_launch(const void*, long long, float*, float*, long long, int, cudaStream_t);
 int gemv_bf16_launch(const void*, const void*, void*, int, int, int, long long, long long, long long, const void*, const void*,
                      long long, int, cudaStream_t);
@@ -355,6 +359,18 @@ int cb_adamw_host(float* p, float* m, float* v, const void* g, void* p16, int64_
                   float eps, float weight_decay, int step, float grad_scale, const float* clip_coef, int ctas, void* stream) {
   return cb::adamw_host_launch(p, m, v, g, p16, n, lr, beta1, beta2, eps, weight_decay, step, grad_scale, clip_coef, ctas,
                                ST(stream));
+}
+int cb_adamw8(float* p, uint8_t* qm, uint8_t* qv, float* sm, float* sv, const void* g, void* p16, int64_t n, float lr,
+              float beta1, float beta2, float eps, float weight_decay, int step, float grad_scale, const float* clip_coef,
+              int background, void* stream) {
+  return cb::adamw8_launch(p, qm, qv, sm, sv, g, p16, n, lr, beta1, beta2, eps, weight_decay, step, grad_scale, clip_coef,
+                           background, ST(stream));
+}
+int cb_adamw8_host(float* p, uint8_t* qm, uint8_t* qv, float* sm, float* sv, const void* g, void* p16, int64_t n,
+                   float lr, float beta1, float beta2, float eps, float weight_decay, int step, float grad_scale,
+                   const float* clip_coef, int ctas, void* stream) {
+  return cb::adamw8_host_launch(p, qm, qv, sm, sv, g, p16, n, lr, beta1, beta2, eps, weight_decay, step, grad_scale,
+                                clip_coef, ctas, ST(stream));
 }
 int cb_embed_grad_sorted(const void* dout, const int64_t* keys, const int32_t* order, void* d_embed, int64_t n, int H,
                          int64_t vocab, void* stream) {

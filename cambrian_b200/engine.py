@@ -25,7 +25,11 @@ buffers for bf16 gradients, fp32 master weights and fp32 Adam moments:
     Without clipping each bucket is updated as soon as it is reduced, under the rest of backward;
   * `offload_optimizer=True` (DeepSpeed's `offload_optimizer`, scripts/zero3_offload.json) keeps the fp32 master and
     moments in registered host memory: the device holds 4 B per trainable parameter instead of 16, and the update kernel
-    (`ops.adamw_host`) streams the state over PCIe, same arithmetic on the GPU, same schedule and streams as above.
+    (`ops.adamw_host`) streams the state over PCIe, same arithmetic on the GPU, same schedule and streams as above;
+  * `optim="adamw_bnb_8bit"` (HF's name, cambrian_trainer.py:365-380) keeps both Adam moments as 8-bit codes with one fp32
+    scale per 256-element block (adam8bit.py states the format): 6.03 instead of 12 optimizer bytes per element.  Parameter
+    offsets are then 256-aligned and buckets padded to 256 * world elements, so no block straddles a parameter, a ZeRO-2
+    piece or a collective slice; embeddings and parameters under 4096 elements keep fp32 moments and the fp32 kernels.
 
 Gradient contributions are counted per parameter: the counts are structural (one per weight-gradient GEMM site, lm_head
 notifies once per step however many row chunks it processes), learned on the first step and verified equal across ranks
@@ -42,7 +46,7 @@ import weakref
 import torch
 import torch.distributed as dist
 
-from . import ops
+from . import adam8bit, ops
 
 
 def _round_up(n: int, m: int) -> int:
@@ -77,9 +81,12 @@ class TrainEngine:
                  weight_decay: float = 0.0, bucket_mb: float = 256.0, process_group=None, overlap: bool = True,
                  zero_stage: int = 0, max_grad_norm: float | None = None, mm_projector_lr: float | None = None,
                  mm_vision_sampler_lr: float | None = None, lr_lambda=None, loss_scale: float = 1.0,
-                 background_optimizer: bool = False, collective: str = "nccl", offload_optimizer: bool = False):
+                 background_optimizer: bool = False, collective: str = "nccl", offload_optimizer: bool = False,
+                 optim: str = "adamw_torch"):
         if zero_stage not in (0, 2):
             raise ValueError("zero_stage must be 0 or 2")
+        self.optim = optim
+        self.eight_bit = adam8bit.resolve_optim(optim)
         if hasattr(model, "check_trainable"):   # a model that trains only in some configurations refuses the others
             model.check_trainable()
         from .quant import quantized_format
@@ -127,16 +134,20 @@ class TrainEngine:
             decay = weight_decay if (id(p) not in norm_params and "bias" not in n) else 0.0
             self.hparams.append((glr, decay))
         # ---- flat layout + buckets: contiguous parameter ranges of ~bucket_mb; with ZeRO-2 every bucket is padded to a
-        #      multiple of 8 * world elements so each rank owns an equal, 16-byte aligned piece of it
+        #      multiple of 8 * world elements so each rank owns an equal, 16-byte aligned piece of it.  With 8-bit moments
+        #      every parameter starts on a 256-element block and every bucket is a multiple of 256 * world elements
         self.collective = collective if (self.world > 1 and zero_stage == 0) else "nccl"
         align = 8 * self.world if (zero_stage == 2 or self.collective != "nccl") else 8
+        palign = 8
+        if self.eight_bit:
+            align, palign = adam8bit.BLOCK * self.world, adam8bit.BLOCK
         limit = int(bucket_mb * 1024 * 1024 / 2)
         offs, total = [], 0
         self.buckets = []      # (start_elem, end_elem, [param indices])
         cur, cur_start = [], 0
         for i, p in enumerate(self.params):
             offs.append(total)
-            total += _round_up(p.numel(), 8)
+            total += _round_up(p.numel(), palign)
             cur.append(i)
             if total - cur_start >= limit:
                 total = _round_up(total - cur_start, align) + cur_start
@@ -178,6 +189,7 @@ class TrainEngine:
         self.offload = bool(offload_optimizer)
         self._closed = False
         self._host_finalizer = None
+        self._host_tensors = []
         self.piece_base = None
         if zero_stage == 2:
             self.piece_base, n_state = [], 0
@@ -196,8 +208,12 @@ class TrainEngine:
             n_state = total
             if not self.offload:
                 self.master = self.flat_p.float()
+        if self.eight_bit:
+            self._init_8bit_layout(model)
         if self.offload:
             self._init_host_state(n_state)
+        elif self.eight_bit:
+            self._init_8bit_moments(dev)
         else:
             self.exp_avg = torch.zeros(n_state, dtype=torch.float32, device=dev)
             self.exp_avg_sq = torch.zeros(n_state, dtype=torch.float32, device=dev)
@@ -235,12 +251,16 @@ class TrainEngine:
         The master is filled one bucket (ZeRO-2: one piece) at a time through a device scratch of that size: a full-size
         fp32 copy on the device is exactly what offloading exists to avoid."""
         self.master = torch.empty(n_state, dtype=torch.float32)
-        self.exp_avg = torch.zeros(n_state, dtype=torch.float32)
-        self.exp_avg_sq = torch.zeros(n_state, dtype=torch.float32)
+        if self.eight_bit:
+            self._init_8bit_moments(torch.device("cpu"))
+        else:
+            self.exp_avg = torch.zeros(n_state, dtype=torch.float32)
+            self.exp_avg_sq = torch.zeros(n_state, dtype=torch.float32)
+        self._host_tensors = [t for t in (self.master, self.exp_avg, self.exp_avg_sq) + self._code_state() if t.numel()]
         if self.flat_p.is_cuda:
             registered = []
             try:
-                for t in (self.master, self.exp_avg, self.exp_avg_sq):
+                for t in self._host_tensors:
                     registered.append(ops.host_register(t))
             except Exception:
                 _release_host_state(self.flat_p.device, registered)
@@ -255,6 +275,48 @@ class TrainEngine:
             sc.copy_(self.flat_p[lo:hi])
             self.master[at:at + hi - lo].copy_(sc)
 
+    def _init_8bit_layout(self, model):
+        """Which parameters keep fp32 moments, and where each parameter's part of this rank's state starts in the fp32
+        moments or in the codes: both are packed in flat order, so 8-bit parameters hold no fp32 moment bytes and
+        fp32-moment parameters no code bytes."""
+        emb = adam8bit.embedding_params(model)
+        self._fp32m = [adam8bit.fp32_moments(p, emb) for p in self.params]
+        self._moff = {}                                 # (bucket, parameter) -> moment offset of its first local element
+        n = {True: 0, False: 0}
+        for b in range(len(self.buckets)):
+            for i in self.buckets[b][2]:
+                lo, hi = self._local_span(b, i)
+                if hi > lo:
+                    self._moff[(b, i)] = n[self._fp32m[i]]
+                    n[self._fp32m[i]] += hi - lo
+        self._n32, self._n8 = n[True], n[False]
+
+    def _init_8bit_moments(self, dev):
+        """fp32 moments of the fp32-moment parameters; codes (m: the signed map's 0.0, v: the unsigned map's) and per-block
+        absmax of the 8-bit ones."""
+        nb = self._n8 // adam8bit.BLOCK
+        self.exp_avg = torch.zeros(self._n32, dtype=torch.float32, device=dev)
+        self.exp_avg_sq = torch.zeros(self._n32, dtype=torch.float32, device=dev)
+        self.exp_avg_code = torch.full((self._n8,), int(torch.nonzero(adam8bit.signed_map() == 0)), dtype=torch.uint8,
+                                       device=dev)
+        self.exp_avg_sq_code = torch.zeros(self._n8, dtype=torch.uint8, device=dev)
+        self.exp_avg_absmax = torch.zeros(nb, dtype=torch.float32, device=dev)
+        self.exp_avg_sq_absmax = torch.zeros(nb, dtype=torch.float32, device=dev)
+
+    def _code_state(self):
+        if not self.eight_bit:
+            return ()
+        return self.exp_avg_code, self.exp_avg_sq_code, self.exp_avg_absmax, self.exp_avg_sq_absmax
+
+    def _local_span(self, b, i):
+        """[lo, hi) of parameter i inside this rank's state range of bucket b, 8-bit mode: an 8-bit parameter covers whole
+        blocks (its padding is zero and stays zero), a fp32-moment one its 8-aligned length, as in the default mode."""
+        lo_p, hi_p = self._piece(b) if self.zero_stage == 2 else self.buckets[b][:2]
+        n = self.params[i].numel()
+        lo = self.offsets[i]
+        hi = lo + _round_up(n, 8 if self._fp32m[i] else adam8bit.BLOCK)
+        return max(lo, lo_p), min(hi, hi_p)
+
     # ---- layout helpers --------------------------------------------------------------------------------------------
     def _piece(self, b):
         s, e, _ = self.buckets[b]
@@ -264,6 +326,8 @@ class TrainEngine:
     def _segments(self, b, skip):
         """Maximal runs [lo, hi) of bucket b with equal (lr, weight decay), leaving out parameters in `skip` (no gradient
         this step: torch.optim skips them entirely)."""
+        if self.eight_bit:
+            return self._segments8(b, skip)
         s, e, idx = self.buckets[b]
         segs = []
         for i in idx:
@@ -276,6 +340,21 @@ class TrainEngine:
                 segs[-1] = (segs[-1][0], hi, hp)
             else:
                 segs.append((lo, hi, hp))
+        return segs
+
+    def _segments8(self, b, skip):
+        """8-bit mode: maximal runs (lo, hi, (lr, wd), fp32 moments, moment offset of lo) of this rank's part of bucket b
+        with equal hyper-parameters and state format, already clipped to the rank's piece."""
+        segs = []
+        for i in self.buckets[b][2]:
+            if i in skip or (b, i) not in self._moff:
+                continue
+            lo, hi = self._local_span(b, i)
+            hp, f32 = self.hparams[i], self._fp32m[i]
+            if segs and segs[-1][1] == lo and segs[-1][2] == hp and segs[-1][3] == f32:
+                segs[-1] = (segs[-1][0], hi, hp, f32, segs[-1][4])
+            else:
+                segs.append((lo, hi, hp, f32, self._moff[(b, i)]))
         return segs
 
     # ---- per-step protocol ---------------------------------------------------------------------------------------
@@ -376,13 +455,16 @@ class TrainEngine:
         coef = self._coef if self.max_grad_norm is not None else None
 
         def run():
-            for (lo, hi, (glr, wd)) in segs:
-                lo, hi = max(lo, lo_p), min(hi, hi_p)
-                if hi <= lo:
-                    continue
-                self._adamw(self.master[state0 + lo:state0 + hi], self.exp_avg[state0 + lo:state0 + hi],
-                            self.exp_avg_sq[state0 + lo:state0 + hi], g[lo - g0:hi - g0], self.flat_p[lo:hi],
-                            glr * mult, wd, self.step_count + 1, coef)
+            if self.eight_bit:
+                self._run_segments8(segs, state0, g, g0, mult, coef)
+            else:
+                for (lo, hi, (glr, wd)) in segs:
+                    lo, hi = max(lo, lo_p), min(hi, hi_p)
+                    if hi <= lo:
+                        continue
+                    self._adamw(self.master[state0 + lo:state0 + hi], self.exp_avg[state0 + lo:state0 + hi],
+                                self.exp_avg_sq[state0 + lo:state0 + hi], g[lo - g0:hi - g0], self.flat_p[lo:hi],
+                                glr * mult, wd, self.step_count + 1, coef)
             if self.zero_stage == 2 and self.world > 1:
                 # in-place all-gather: this rank's piece already sits at its slot of the bucket (NCCL's in-place layout)
                 src = self.flat_p[lo_p:hi_p]
@@ -402,6 +484,24 @@ class TrainEngine:
                     run()
             else:
                 run()
+
+    def _run_segments8(self, segs, state0, g, g0, mult, coef):
+        step = self.step_count + 1
+        for (lo, hi, (glr, wd), f32, mo) in segs:
+            master, p16, gs = self.master[state0 + lo:state0 + hi], self.flat_p[lo:hi], g[lo - g0:hi - g0]
+            n = hi - lo
+            if f32:
+                self._adamw(master, self.exp_avg[mo:mo + n], self.exp_avg_sq[mo:mo + n], gs, p16, glr * mult, wd, step,
+                            coef)
+                continue
+            b0, nb = mo // adam8bit.BLOCK, adam8bit.blocks(n)
+            args = (master, self.exp_avg_code[mo:mo + n], self.exp_avg_sq_code[mo:mo + n],
+                    self.exp_avg_absmax[b0:b0 + nb], self.exp_avg_sq_absmax[b0:b0 + nb], gs, p16, glr * mult,
+                    self.betas[0], self.betas[1], self.eps, wd, step)
+            if self.offload:
+                ops.adamw8_host(*args, grad_scale=1.0 / self.world, clip_coef=coef)
+            else:
+                ops.adamw8(*args, grad_scale=1.0 / self.world, clip_coef=coef, background=self.background)
 
     def _adamw(self, master, m, v, g, p16, lr, wd, step, coef):
         if self.offload:
@@ -569,12 +669,18 @@ class TrainEngine:
         return out.loss
 
     def state_bytes(self):
-        """Device bytes of training state: bf16 weights and gradients, plus the fp32 master and moments unless offloaded."""
+        """Device bytes of training state: bf16 weights and gradients, plus the fp32 master and the moments (fp32, or 8-bit
+        codes and block scales) unless offloaded."""
+        if self.eight_bit:
+            opt = sum(t.numel() * t.element_size() for t in (self.master, self.exp_avg, self.exp_avg_sq) + self._code_state())
+            return self.total * 4 + (0 if self.offload else opt)
         opt = (self.shard if self.zero_stage == 2 else self.total) * 12
         return self.total * 4 + (0 if self.offload else opt)
 
     def host_state_bytes(self):
-        """Host bytes of the offloaded fp32 master and moments (0 without offload_optimizer)."""
+        """Host bytes of the offloaded master and moments (0 without offload_optimizer)."""
+        if self.eight_bit:
+            return sum(t.numel() * t.element_size() for t in self._host_tensors) if self.offload else 0
         return 3 * 4 * self.master.numel() if self.offload else 0
 
     def close(self):

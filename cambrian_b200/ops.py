@@ -597,6 +597,23 @@ def adamw_host(p32, m, v, g16, p16, lr, beta1, beta2, eps, wd, step: int, grad_s
                                     int(ctas), stream()), "cb_adamw_host")
 
 
+def adamw8(p32, qm, qv, sm, sv, g16, p16, lr, beta1, beta2, eps, wd, step: int, grad_scale: float = 1.0, clip_coef=None,
+           background: bool = False):
+    """`adamw` with 8-bit block-wise moments (adam8bit.py states the format): qm / qv uint8 codes (one per element), sm /
+    sv fp32 absmax per 256-element block (ceil(n / 256) each); p32 stays the fp32 master."""
+    check(_lib.load().cb_adamw8(ptr(p32), ptr(qm), ptr(qv), ptr(sm), ptr(sv), ptr(g16), ptr(p16), p32.numel(), float(lr),
+                                float(beta1), float(beta2), float(eps), float(wd), int(step), float(grad_scale),
+                                ptr(clip_coef), int(background), stream()), "cb_adamw8")
+
+
+def adamw8_host(p32, qm, qv, sm, sv, g16, p16, lr, beta1, beta2, eps, wd, step: int, grad_scale: float = 1.0,
+                clip_coef=None, ctas: int = 0):
+    """`adamw8` with p32, qm, qv, sm, sv in host memory registered by `host_register` (bitwise equal to `adamw8`)."""
+    check(_lib.load().cb_adamw8_host(ptr(p32), ptr(qm), ptr(qv), ptr(sm), ptr(sv), ptr(g16), ptr(p16), p32.numel(),
+                                     float(lr), float(beta1), float(beta2), float(eps), float(wd), int(step),
+                                     float(grad_scale), ptr(clip_coef), int(ctas), stream()), "cb_adamw8_host")
+
+
 _HOST_REGISTER_PORTABLE, _HOST_REGISTER_MAPPED = 1, 2
 
 

@@ -28,13 +28,17 @@ NF4_CODE = (-1.0, -0.6961928009986877, -0.5250730514526367, -0.39491748809814453
 PROJECTIONS = ("q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj")
 
 
-def dynamic_map() -> torch.Tensor:
-    """bitsandbytes `create_dynamic_map(signed=True)`: 256 sorted fp32 values."""
+def dynamic_map(signed: bool = True) -> torch.Tensor:
+    """bitsandbytes `create_dynamic_map(signed)`: 256 sorted fp32 values.  Both hold 0 and 1.0; decade i = 0..6 adds
+    10^(i-6) times the interval means of linspace(0.1, 1, k + 1), with k = 2^i means and their negatives (signed) or
+    k = 2^(i+1) means (unsigned)."""
     data = [0.0, 1.0]
     for i in range(7):
-        b = torch.linspace(0.1, 1, 2 ** i + 1, dtype=torch.float32)
+        b = torch.linspace(0.1, 1, 2 ** (i if signed else i + 1) + 1, dtype=torch.float32)
         means = (b[:-1] + b[1:]) / 2.0
-        data += ((10 ** (i - 6)) * means).tolist() + (-(10 ** (i - 6)) * means).tolist()
+        data += ((10 ** (i - 6)) * means).tolist()
+        if signed:
+            data += (-(10 ** (i - 6)) * means).tolist()
     return torch.tensor(sorted(data), dtype=torch.float32)
 
 

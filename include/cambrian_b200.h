@@ -236,6 +236,20 @@ int cb_adamw_ex(float* p, float* m, float* v, const void* g, void* p16, int64_t 
  * PCIe-bound grid (0 = default); 128-thread blocks without shared memory that fit next to a resident GEMM CTA. */
 int cb_adamw_host(float* p, float* m, float* v, const void* g, void* p16, int64_t n, float lr, float beta1, float beta2,
                   float eps, float weight_decay, int step, float grad_scale, const float* clip_coef, int ctas, void* stream);
+/* cb_adamw_ex with 8-bit block-wise quantised moments (HF `optim="adamw_bnb_8bit"`, cambrian_trainer.py:365-367): m and v
+ * are one uint8 code per element (qm against the signed dynamic map, qv against the unsigned one) and one fp32 absmax per
+ * 256-element block (sm, sv; ceil(n / 256) each); p stays the fp32 master.  Per element: dequantise (map[code] * absmax),
+ * update with cb_adamw_ex's arithmetic, write p and p16; then per block requantise m and v against their new absmax.
+ * n % 8 == 0; the last block may be partial.  No atomics: bit-reproducible.  Alignment: p, g, p16 16 B; qm, qv 8 B. */
+int cb_adamw8(float* p, uint8_t* qm, uint8_t* qv, float* sm, float* sv, const void* g, void* p16, int64_t n, float lr,
+              float beta1, float beta2, float eps, float weight_decay, int step, float grad_scale, const float* clip_coef,
+              int background, void* stream);
+/* cb_adamw8 with p, qm, qv, sm, sv in registered, mapped host memory (offload_optimizer), bitwise equal to cb_adamw8; g,
+ * p16 (and clip_coef) are device memory.  Placement is checked as cb_adamw_host checks it, before any launch.  ctas:
+ * blocks of the PCIe-bound grid (0 = default). */
+int cb_adamw8_host(float* p, uint8_t* qm, uint8_t* qv, float* sm, float* sv, const void* g, void* p16, int64_t n,
+                   float lr, float beta1, float beta2, float eps, float weight_decay, int step, float grad_scale,
+                   const float* clip_coef, int ctas, void* stream);
 /* Deterministic gradient of the embedding rows (backward of embed_tokens inside cb_embed_splice): rows of dout [n, H] with
  * equal keys[t] (token id; >= vocab = no gradient, e.g. the image span) are summed in position order by one block and
  * written once to d_embed [vocab, H] (pre-zeroed).  `order` = positions stably sorted by key.  Replaces the racing
