@@ -67,7 +67,10 @@ int cb_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int
  *   mask[t] : [batch*q_side*q_side, r[t]*r[t]] bool (1 byte) or NULL (= all true); `mask` itself may be NULL
  *   lse : [batch*q_side*q_side, 16] fp32 log2-domain log-sum-exp, needed by the backward (may be NULL)
  *   windowed = 1: k/v are the reference's window-rearranged [N, r*r, hidden] tensors (vision_sampler.py API);
- *   windowed = 0: natural grid layout (the fast path used by cambrian_arch: no permute/contiguous copies) */
+ *   windowed = 0: natural grid layout (the fast path used by cambrian_arch: no permute/contiguous copies)
+ *   A query whose keys are masked in every tower attends to nothing: the forward writes out = 0 and LSE = +inf for it
+ *   (not NaN), and the backward writes dq = 0 for it.  The backward writes every dk / dv row of every tower: masked keys,
+ *   including all keys of such a query, get exact zero rows. */
 int cb_sva_window_attn_fwd(const void* q, void* out, float* lse, int num_towers, const void* const* k,
                            const void* const* v, const void* const* mask, const int* r, int batch,
                            int q_side, int hidden, int windowed, void* stream);

@@ -8,6 +8,8 @@ stand-in computes in fp32 and rounds once to bf16, like the kernels it mirrors (
 """
 from __future__ import annotations
 
+import math
+
 import torch
 import torch.nn.functional as F
 
@@ -99,19 +101,25 @@ def _win(t, batch, q_side, r, windowed, n):
 
 
 def _sva(q, ks, vs, masks, rs, batch, q_side, windowed):
+    """(out [N, 1024], log2-domain LSE [N, 16]).  A query whose keys are all masked attends to nothing: out = 0 and
+    LSE = +inf, as the kernel writes them (its gradients are then 0 too)."""
     n = q.shape[0]
     K = torch.cat([_win(k, batch, q_side, r, windowed, n) for k, r in zip(ks, rs)], 1).view(n, -1, 16, 64).transpose(1, 2)
     V = torch.cat([_win(v, batch, q_side, r, windowed, n) for v, r in zip(vs, rs)], 1).view(n, -1, 16, 64).transpose(1, 2)
-    ms = [torch.ones(n, r * r, dtype=torch.bool) if masks is None or masks[i] is None else masks[i].reshape(n, -1).bool()
-          for i, r in enumerate(rs)]
+    ms = [torch.ones(n, r * r, dtype=torch.bool, device=q.device) if masks is None or masks[i] is None
+          else masks[i].reshape(n, -1).bool() for i, r in enumerate(rs)]
+    keep = torch.cat(ms, 1)[:, None, None, :]
+    any_key = keep.any(-1, keepdim=True)
     s = (q.view(n, 1, 16, 64).transpose(1, 2) @ K.transpose(-1, -2)) / 8.0
-    s = s.masked_fill(~torch.cat(ms, 1)[:, None, None, :], float("-inf"))
-    return (torch.softmax(s, -1) @ V).transpose(1, 2).reshape(n, 1024)
+    s = s.masked_fill(~keep, float("-inf")).masked_fill(~any_key, 0.0)
+    out = ((torch.softmax(s, -1) * any_key) @ V).transpose(1, 2).reshape(n, 1024)
+    lse = (torch.logsumexp(s, -1) / math.log(2.0)).masked_fill(~any_key[..., 0], float("inf")).reshape(n, 16)
+    return out, lse
 
 
 def sva_window_attn_fwd(q, ks, vs, masks, rs, batch, q_side, need_lse=True, windowed=False):
-    out = _sva(q.float(), [k.float() for k in ks], [v.float() for v in vs], masks, rs, batch, q_side, windowed)
-    return out.to(torch.bfloat16), torch.zeros(q.shape[0], 16)
+    out, lse = _sva(q.float(), [k.float() for k in ks], [v.float() for v in vs], masks, rs, batch, q_side, windowed)
+    return out.to(torch.bfloat16), (lse if need_lse else None)
 
 
 def sva_window_attn_bwd(q, out, dout, lse, ks, vs, masks, rs, batch, q_side, windowed=False, dks=None, dvs=None):
@@ -119,7 +127,7 @@ def sva_window_attn_bwd(q, out, dout, lse, ks, vs, masks, rs, batch, q_side, win
     kf = [k.float().requires_grad_() for k in ks]
     vf = [v.float().requires_grad_() for v in vs]
     with torch.enable_grad():
-        o = _sva(qf, kf, vf, masks, rs, batch, q_side, windowed)
+        o = _sva(qf, kf, vf, masks, rs, batch, q_side, windowed)[0]
     gs = [g.to(torch.bfloat16) for g in torch.autograd.grad(o, [qf] + kf + vf, dout.float())]
     T = len(ks)
     gk, gv = gs[1:1 + T], gs[1 + T:]
@@ -171,10 +179,18 @@ def pos_grad(dx, B, side, r, out=None, accumulate=False):
 
 
 def bilinear(x, h, w, th, tw, *, in_bs=None, out=None, out_ld=None, out_col0=0):
+    """rows of a batch are read at batch stride in_bs (default x.stride(0)); with `out`, written at row stride out_ld
+    (default out.stride(1)) from column out_col0 — a column slice of a wider buffer."""
     B, C = x.shape[0], x.shape[-1]
-    y = F.interpolate(x[:, :h * w].float().reshape(B, h, w, C).permute(0, 3, 1, 2), size=(th, tw), mode="bilinear",
+    src = x.as_strided((B, h * w, C), (x.stride(0) if in_bs is None else in_bs, C, 1))
+    y = F.interpolate(src.float().reshape(B, h, w, C).permute(0, 3, 1, 2), size=(th, tw), mode="bilinear",
                       align_corners=False)
-    return y.permute(0, 2, 3, 1).reshape(B, th * tw, C).to(torch.bfloat16)
+    y = y.permute(0, 2, 3, 1).reshape(B, th * tw, C).to(torch.bfloat16)
+    if out is None:
+        return y
+    ld = out.stride(1) if out_ld is None else out_ld
+    out.as_strided((B, th * tw, C), (out.stride(0), ld, 1), out.storage_offset() + out_col0).copy_(y)
+    return out
 
 
 def bilinear_bwd(dout, h, w, th, tw):
