@@ -895,6 +895,15 @@ int attn_bwd_launch(const void* q, const void* k, const void* v, const void* o, 
   CB_CHECK_ARG(lse && delta && dq && dk && dv, "attention bwd: lse / delta / dq / dk / dv buffers are required");
   CB_CHECK_ARG(!(reinterpret_cast<uintptr_t>(dq) & 3u) && dq_bs % 2 == 0 && dq_ss % 2 == 0,
                "attention bwd: dq must be 4-byte aligned with even strides");
+  // dK / dV are stored as bf16 pairs; the delta kernel reads O and dO as 16-byte vectors (O never gets a tensor map)
+  CB_CHECK_ARG(!(reinterpret_cast<uintptr_t>(dk) & 3u) && (B == 1 || dk_bs % 2 == 0) && dk_ss % 2 == 0,
+               "attention bwd: dk must be 4-byte aligned with even strides");
+  CB_CHECK_ARG(!(reinterpret_cast<uintptr_t>(dv) & 3u) && (B == 1 || dv_bs % 2 == 0) && dv_ss % 2 == 0,
+               "attention bwd: dv must be 4-byte aligned with even strides");
+  CB_CHECK_ARG(o && !(reinterpret_cast<uintptr_t>(o) & 15u) && (B == 1 || o_bs % 8 == 0) && o_ss % 8 == 0,
+               "attention bwd: o must be 16-byte aligned with strides %% 8 == 0");
+  CB_CHECK_ARG(d_o && !(reinterpret_cast<uintptr_t>(d_o) & 15u) && (B == 1 || do_bs % 8 == 0) && do_ss % 8 == 0,
+               "attention bwd: d_o must be 16-byte aligned with strides %% 8 == 0");
   {
     const long long warps = ((long long)B * Sq * nh + (256 / hd) - 1) / (256 / hd);   // 32 / (hd / 8) heads per warp
     auto kern = hd == 96 ? attn_delta_kernel<true> : attn_delta_kernel<false>;       // hd 96: 2 heads per warp

@@ -288,6 +288,18 @@ def _bshd_strides(t, hd):
     return t.stride(0), t.stride(1)
 
 
+def _kmask_u8(kmask, B: int, Skv: int):
+    """The key mask as the kernels read it: [B, Skv] contiguous uint8, row b at b * Skv (1 = attend).  A mask over a
+    longer buffer (e.g. the whole [B, S_max] cache while K / V are a prefix of it) would shift every row b >= 1, so it is
+    refused: slice it to the keys the call attends over."""
+    if kmask is None:
+        return None
+    if tuple(kmask.shape) != (B, Skv):
+        raise ValueError(f"attention: kmask must be [B, Skv] = [{B}, {Skv}], got {list(kmask.shape)}")
+    kmask = kmask.contiguous()
+    return kmask.view(torch.uint8) if kmask.dtype == torch.bool else kmask.to(torch.uint8)
+
+
 def attn_fwd(q, k, v, *, causal: bool, kmask=None, scale: float | None = None, need_lse: bool = False, out=None,
              window: int = 0):
     """q [B,Sq,nh,hd], k/v [B,Skv,nkv,hd] (views are fine) -> o [B,Sq,nh,hd] contiguous (+ lse [B,nh,Sq]).
@@ -304,9 +316,7 @@ def attn_fwd(q, k, v, *, causal: bool, kmask=None, scale: float | None = None, n
     kb, ks = _bshd_strides(k, hd)
     vb, vs_ = _bshd_strides(v, hd)
     ob, os_ = _bshd_strides(o, hd)
-    if kmask is not None:
-        kmask = kmask.contiguous()
-        kmask = kmask.view(torch.uint8) if kmask.dtype == torch.bool else kmask.to(torch.uint8)
+    kmask = _kmask_u8(kmask, B, Skv)
     if window:
         rc = _lib.load().cb_attn_fwd_window(ptr(q), ptr(k), ptr(v), ptr(o), ptr(lse), ptr(kmask), B, nh, nkv, Sq, Skv,
                                             hd, qb, qs, kb, ks, vb, vs_, ob, os_, float(scale), int(causal), int(window),
@@ -341,9 +351,7 @@ def attn_bwd(q, k, v, o, do, lse, *, causal: bool, kmask=None, scale: float | No
     dqb, dqs = _bshd_strides(dq, hd)
     dkb, dks = _bshd_strides(dk, hd)
     dvb, dvs = _bshd_strides(dv, hd)
-    if kmask is not None:
-        kmask = kmask.contiguous()
-        kmask = kmask.view(torch.uint8) if kmask.dtype == torch.bool else kmask.to(torch.uint8)
+    kmask = _kmask_u8(kmask, B, Skv)
     if window:
         rc = _lib.load().cb_attn_bwd_window(ptr(q), ptr(k), ptr(v), ptr(o), ptr(do), ptr(lse), ptr(delta), ptr(dq),
                                             ptr(dk), ptr(dv), ptr(kmask), B, nh, nkv, Sq, Skv, hd, qb, qs, kb, ks, vb,

@@ -287,44 +287,73 @@ def rope_(buf, pos, cos_t, sin_t, n_heads, hd, inverse=False):
     return buf
 
 
-def _attn(q, k, v, causal, kmask, scale):
+def attn_visible(Sq, Skv, causal, window=0, kmask=None, device=None):
+    """[B or 1, Sq, Skv] bool: query row r (slot i = r + Skv - Sq) sees key j iff j <= i when causal, i - j < window when
+    window > 0, and kmask[b, j]."""
+    i = torch.arange(Sq, device=device)[:, None] + (Skv - Sq)
+    j = torch.arange(Skv, device=device)[None, :]
+    vis = torch.ones(Sq, Skv, dtype=torch.bool, device=device)
+    if causal:
+        vis = vis & (j <= i)
+    if window:
+        vis = vis & (i - j < window)
+    vis = vis[None]
+    if kmask is not None:
+        vis = vis & kmask.bool()[:, None, :]
+    return vis
+
+
+def _attn_scores(q, k, causal, kmask, scale, window):
+    """fp32 scores [B, nh, Sq, Skv] (K repeated over the GQA group) with hidden pairs at -inf, and the visibility."""
     B, Sq, nh, hd = q.shape
     Skv, nkv = k.shape[1], k.shape[2]
-    Q = q.transpose(1, 2)
-    K = k.transpose(1, 2).repeat_interleave(nh // nkv, 1)
-    V = v.transpose(1, 2).repeat_interleave(nh // nkv, 1)
-    s = Q @ K.transpose(-1, -2) * (scale if scale is not None else hd ** -0.5)
-    allow = torch.ones(Sq, Skv, dtype=torch.bool)
-    if causal:
-        allow = allow.tril(Skv - Sq)
-    allow = allow[None, None]
-    if kmask is not None:
-        allow = allow & kmask.bool()[:, None, None, :]
-    p = torch.nan_to_num(torch.softmax(s.masked_fill(~allow, float("-inf")), -1), 0.0)
-    return (p @ V).transpose(1, 2)
+    K = k.float().transpose(1, 2).repeat_interleave(nh // nkv, 1)
+    s = q.float().transpose(1, 2) @ K.transpose(-1, -2) * (scale if scale is not None else hd ** -0.5)
+    vis = attn_visible(Sq, Skv, causal, window, kmask, q.device)[:, None]
+    return s.masked_fill(~vis, float("-inf")), vis
 
 
-def attn_fwd(q, k, v, *, causal, kmask=None, scale=None, need_lse=False, out=None):
-    o = _attn(q.float(), k.float(), v.float(), causal, kmask, scale).to(torch.bfloat16).contiguous()
-    if out is not None:
-        out.copy_(o)
-        o = out
-    return (o, torch.zeros(q.shape[0], q.shape[2], q.shape[1])) if need_lse else o
+def _store_into(g, dst):
+    g = g.to(torch.bfloat16)
+    if dst is None:
+        return g.contiguous()
+    dst.copy_(g)
+    return dst
 
 
-def attn_bwd(q, k, v, o, do, lse, *, causal, kmask=None, scale=None, dq=None, dk=None, dv=None):
-    qf, kf, vf = (t.float().detach().requires_grad_() for t in (q, k, v))
-    with torch.enable_grad():
-        out = _attn(qf, kf, vf, causal, kmask, scale)
-    gq, gk, gv = torch.autograd.grad(out, [qf, kf, vf], do.float())
-    res = []
-    for g, dst in ((gq, dq), (gk, dk), (gv, dv)):
-        g = g.to(torch.bfloat16)
-        if dst is not None:
-            dst.copy_(g)
-            g = dst
-        res.append(g)
-    return tuple(res)
+def attn_fwd(q, k, v, *, causal, kmask=None, scale=None, need_lse=False, out=None, window=0):
+    """O and the log2-domain LSE of the scaled scores; a row that sees no key gets O = 0 and LSE = +inf, as the kernel
+    writes them."""
+    B, Sq, nh, hd = q.shape
+    s, vis = _attn_scores(q, k, causal, kmask, scale, window)
+    live = vis.any(-1, keepdim=True)
+    p = torch.softmax(s.masked_fill(~live, 0.0), -1) * live
+    V = v.float().transpose(1, 2).repeat_interleave(nh // k.shape[2], 1)
+    o = _store_into((p @ V).transpose(1, 2), out)
+    if not need_lse:
+        return o
+    lse = (torch.logsumexp(s.masked_fill(~live, 0.0), -1) / math.log(2.0)).masked_fill(~live[..., 0], float("inf"))
+    return o, lse
+
+
+def attn_bwd(q, k, v, o, do, lse, *, causal, kmask=None, scale=None, dq=None, dk=None, dv=None, window=0):
+    """The kernels' closed form: P = exp2(S log2(e) - LSE) from the forward's LSE, delta = rowsum(dO * O) from the stored
+    O, dS = P (dO V^T - delta), dQ = scale dS K, dK = scale dS^T Q and dV = P^T dO summed over the GQA group."""
+    B, Sq, nh, hd = q.shape
+    Skv, nkv = k.shape[1], k.shape[2]
+    G = nh // nkv
+    sc = scale if scale is not None else hd ** -0.5
+    s, vis = _attn_scores(q, k, causal, kmask, sc, window)
+    L = lse.float()[..., None]
+    p = torch.exp2(s * (1.0 / math.log(2.0)) - L.masked_fill(torch.isinf(L), 0.0)).masked_fill(~vis | torch.isinf(L), 0.0)
+    Q, dO = q.float().transpose(1, 2), do.float().transpose(1, 2)
+    K = k.float().transpose(1, 2).repeat_interleave(G, 1)
+    V = v.float().transpose(1, 2).repeat_interleave(G, 1)
+    delta = (dO * o.float().transpose(1, 2)).sum(-1, keepdim=True)
+    ds = p * (dO @ V.transpose(-1, -2) - delta)
+    group = lambda t: t.view(B, nkv, G, Skv, hd).sum(2).transpose(1, 2)
+    return (_store_into((ds @ K * sc).transpose(1, 2), dq), _store_into(group(ds.transpose(-1, -2) @ Q * sc), dk),
+            _store_into(group(p.transpose(-1, -2) @ dO), dv))
 
 
 def swiglu_fwd(gate, up):

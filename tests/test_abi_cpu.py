@@ -109,3 +109,33 @@ def test_resample_coefficients_are_normalised(lib):
             assert 0 <= x0 and x0 + n <= src and 0 < n <= ks
             row = kk[x * ks:(x + 1) * ks]
             assert abs(sum(row) - (1 << 22)) <= ks and all(v == 0 for v in row[n:])
+
+
+def test_attention_backward_refuses_misaligned_operands_without_gpu(lib):
+    """O and dO are read as 16-byte vectors by the delta kernel, dK and dV stored as bf16 pairs: a misaligned pointer or
+    stride is refused before the first launch (fake, never dereferenced pointers)."""
+    B, nh, nkv, S, hd = 2, 4, 2, 128, 64
+    rs, bs = nh * hd, S * nh * hd                                   # packed heads: row and batch strides of a [B, S, nh, hd]
+    ks, kbs = nkv * hd, S * nkv * hd
+    base = 1 << 20
+
+    def call(o=base, d_o=base, dk=base, dv=base, o_ss=rs, o_bs=bs, do_ss=rs, do_bs=bs, dk_ss=ks, dk_bs=kbs, dv_ss=ks,
+             dv_bs=kbs, Bn=B):
+        p = ctypes.c_void_p
+        return lib.cb_attn_bwd(p(base), p(base), p(base), p(o), p(d_o), p(base), p(base), p(base), p(dk), p(dv), None,
+                               Bn, nh, nkv, S, S, hd, bs, rs, kbs, ks, kbs, ks, o_bs, o_ss, do_bs, do_ss, bs, rs, dk_bs,
+                               dk_ss, dv_bs, dv_ss, ctypes.c_float(0.125), 1, None)
+
+    for kw, name in ((dict(o=base + 2), b"o must"), (dict(o=base + 8), b"o must"), (dict(o_ss=rs + 4), b"o must"),
+                     (dict(o_bs=bs + 2), b"o must"), (dict(d_o=base + 8), b"d_o must"), (dict(do_ss=rs + 2), b"d_o must"),
+                     (dict(do_bs=bs + 4), b"d_o must"), (dict(dk=base + 2), b"dk must"), (dict(dk_ss=ks + 1), b"dk must"),
+                     (dict(dk_bs=kbs + 1), b"dk must"), (dict(dv=base + 6), b"dv must"), (dict(dv_ss=ks + 1), b"dv must"),
+                     (dict(dv_bs=kbs - 1), b"dv must"), (dict(o=0), b"o must")):
+        assert call(**kw) == 1, kw
+        assert name in lib.cb_last_error(), (kw, lib.cb_last_error())
+    # a single batch element never uses its batch stride
+    assert call(Bn=1, o=base + 2) == 1
+    rc = lib.cb_attn_bwd_window(*([ctypes.c_void_p(base)] * 4 + [ctypes.c_void_p(base + 8)] + [ctypes.c_void_p(base)] * 5
+                                  + [None]), B, nh, nkv, S, S, hd, bs, rs, kbs, ks, kbs, ks, bs, rs, bs, rs, bs, rs, kbs, ks,
+                                kbs, ks, ctypes.c_float(0.125), 1, 64, None)
+    assert rc == 1 and b"d_o must" in lib.cb_last_error()

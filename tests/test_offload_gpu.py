@@ -162,6 +162,10 @@ def test_offload_memory_accounting_and_lifetime():
     engines = {}
     for offload in (False, True):
         cfg, model, batch = _setup()
+        # the engine moves every parameter into its flat buffer and frees the old storage; keeping that storage alive until
+        # the engine is measured leaves the count to the engine's own allocations (the blocks the freed parameters held
+        # depend on what the caching allocator had cached when the model was built)
+        old_storage = [p.data for p in model.parameters()]
         torch.cuda.synchronize()
         torch.cuda.reset_peak_memory_stats()
         before = torch.cuda.memory_allocated()
@@ -169,6 +173,7 @@ def test_offload_memory_accounting_and_lifetime():
         torch.cuda.synchronize()
         used[offload] = (torch.cuda.memory_allocated() - before, torch.cuda.max_memory_allocated() - before)
         engines[offload] = (eng, model, batch)
+        del old_storage
     ref, eng = engines[False][0], engines[True][0]
     n_state = eng.master.numel()
     assert n_state == eng.total and len(eng.buckets) > 3

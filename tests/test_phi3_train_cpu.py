@@ -24,51 +24,23 @@ GOLD = os.path.join(HERE, "golden")
 W, S, VALID = 5, 12, 7          # the second row has VALID tokens: at W = 5 its query slots 11.. see no key
 
 
-def _attn(q, k, v, kmask, scale, window):
-    """fp32 attention under the oracle's mask; a row that sees no key gives zeros (and zero gradients)."""
-    B, Sq, nh, hd = q.shape
-    Skv, nkv = k.shape[1], k.shape[2]
-    Q = q.transpose(1, 2)
-    K = k.transpose(1, 2).repeat_interleave(nh // nkv, 1)
-    V = v.transpose(1, 2).repeat_interleave(nh // nkv, 1)
-    s = Q @ K.transpose(-1, -2) * (scale if scale is not None else hd ** -0.5)
-    allow = P.sliding_mask(Sq, Skv, window, kmask)[:, None]
-    live = allow.any(-1, keepdim=True)
-    p = torch.softmax(s.masked_fill(~allow, float("-inf")).masked_fill(~live, 0.0), -1).masked_fill(~live, 0.0)
-    return (p @ V).transpose(1, 2)
-
-
 def _install(monkeypatch, calls):
-    """ops_emulation plus windowed attn_fwd / attn_bwd stand-ins that record the window of every call; the CUDA-bf16
-    training guard is lifted so the CPU model trains."""
+    """ops_emulation, with its attn_fwd / attn_bwd wrapped to record the window of every call; the CUDA-bf16 training
+    guard is lifted so the CPU model trains."""
     from cambrian_b200 import ops
     from cambrian_b200.model.language_model import cambrian_phi3
     ops_emulation.install(monkeypatch)
     monkeypatch.setattr(cambrian_phi3, "require_cuda_bf16", lambda model: None)
 
-    def attn_fwd(q, k, v, *, causal, kmask=None, scale=None, need_lse=False, out=None, window=0):
-        assert causal
-        calls.append(("fwd", window))
-        o = _attn(q.float(), k.float(), v.float(), kmask, scale, window).to(torch.bfloat16).contiguous()
-        if out is not None:
-            out.copy_(o)
-            o = out
-        return (o, torch.zeros(q.shape[0], q.shape[2], q.shape[1])) if need_lse else o
+    def recording(kind, fn):
+        def wrapped(*args, causal, window=0, **kw):
+            assert causal
+            calls.append((kind, window))
+            return fn(*args, causal=causal, window=window, **kw)
+        return wrapped
 
-    def attn_bwd(q, k, v, o, do, lse, *, causal, kmask=None, scale=None, dq=None, dk=None, dv=None, window=0):
-        assert causal
-        calls.append(("bwd", window))
-        qf, kf, vf = (t.float().detach().requires_grad_() for t in (q, k, v))
-        with torch.enable_grad():
-            out = _attn(qf, kf, vf, kmask, scale, window)
-        res = []
-        for g, dst in zip(torch.autograd.grad(out, [qf, kf, vf], do.float()), (dq, dk, dv)):
-            dst.copy_(g.to(torch.bfloat16))
-            res.append(dst)
-        return tuple(res)
-
-    monkeypatch.setattr(ops, "attn_fwd", attn_fwd)
-    monkeypatch.setattr(ops, "attn_bwd", attn_bwd)
+    monkeypatch.setattr(ops, "attn_fwd", recording("fwd", ops_emulation.attn_fwd))
+    monkeypatch.setattr(ops, "attn_bwd", recording("bwd", ops_emulation.attn_bwd))
 
 
 def _batch(vocab):
