@@ -98,6 +98,9 @@ SIGNATURES = {
     "cb_fp8_quantize_weight_t": (_i, [_vp, _i, _i, _i64, _vp, _vp, _vp, _i64, _vp]),
     "cb_rmsnorm_fwd_fp8": (_i, [_vp] * 5 + [_i64, _i, _f, _i, _vp]),
     "cb_swiglu_bwd_fp8": (_i, [_vp] * 7 + [_i64, _i, _i64, _i64, _i64, _vp]),
+    "cb_paged_kv_append": (_i, [_vp, _vp, _i64] + [_vp] * 4 + [_i, _vp, _i64, _vp] + [_i] * 7 + [_i64, _i, _vp]),
+    "cb_attn_decode_paged_workspace_floats": (_i64, [_i] * 5),
+    "cb_attn_decode_paged": (_i, [_vp, _i64] + [_vp] * 4 + [_i, _vp, _i64, _vp, _i, _vp, _vp, _i64] + [_i] * 7 + [_f, _vp]),
 }
 
 _lib = None

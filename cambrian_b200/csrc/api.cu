@@ -140,6 +140,12 @@ int fp8_quantize_weight_t_launch(const void*, int, int, long long, void*, float*
 int rmsnorm_fwd_fp8(const void*, const void*, void*, float*, float*, long long, int, float, int, cudaStream_t);
 int swiglu_bwd_fp8_launch(const void*, const void*, const void*, void*, void*, void*, float*, long long, int, long long,
                           long long, long long, cudaStream_t);
+int paged_kv_append_launch(const void*, const void*, long long, void*, void*, float*, float*, int, const int*, long long,
+                           const int*, int, int, int, int, int, int, int, long long, int, cudaStream_t);
+long long attn_decode_paged_workspace_floats(int, int, int, int, int);
+int attn_decode_paged_launch(const void*, long long, const void*, const void*, const float*, const float*, int, const int*,
+                             long long, const int*, int, void*, float*, long long, int, int, int, int, int, int, int, float,
+                             cudaStream_t);
 
 }  // namespace cb
 
@@ -481,6 +487,24 @@ int cb_rmsnorm_fwd_fp8(const void* x, const void* gamma, void* xq, float* sa, fl
 int cb_swiglu_bwd_fp8(const void* dout, const void* gate, const void* up, void* dgate, void* dup, void* dguq, float* sdgu,
                       int64_t rows, int I, int64_t ld_in, int64_t ld_dout, int64_t ld_dgu, void* stream) {
   return cb::swiglu_bwd_fp8_launch(dout, gate, up, dgate, dup, dguq, sdgu, rows, I, ld_in, ld_dout, ld_dgu, ST(stream));
+}
+int cb_paged_kv_append(const void* k, const void* v, int64_t ld, void* k_pages, void* v_pages, float* k_scales,
+                       float* v_scales, int fp8, const int* block_table, int64_t table_ld, const int* lens, int rows, int S,
+                       int nkv, int hd, int page_size, int num_pages, int max_pages, int64_t offset, int offset_from_lens,
+                       void* stream) {
+  return cb::paged_kv_append_launch(k, v, ld, k_pages, v_pages, k_scales, v_scales, fp8, block_table, table_ld, lens, rows,
+                                    S, nkv, hd, page_size, num_pages, max_pages, offset, offset_from_lens, ST(stream));
+}
+int64_t cb_attn_decode_paged_workspace_floats(int rows, int nh, int max_pages, int page_size, int hd) {
+  return cb::attn_decode_paged_workspace_floats(rows, nh, max_pages, page_size, hd);
+}
+int cb_attn_decode_paged(const void* q, int64_t q_bs, const void* k_pages, const void* v_pages, const float* k_scales,
+                         const float* v_scales, int fp8, const int* block_table, int64_t table_ld, const int* lens,
+                         int len_add, void* o, float* workspace, int64_t workspace_floats, int rows, int nh, int nkv, int hd,
+                         int page_size, int num_pages, int max_pages, float scale, void* stream) {
+  return cb::attn_decode_paged_launch(q, q_bs, k_pages, v_pages, k_scales, v_scales, fp8, block_table, table_ld, lens,
+                                      len_add, o, workspace, workspace_floats, rows, nh, nkv, hd, page_size, num_pages,
+                                      max_pages, scale, ST(stream));
 }
 
 }  // extern "C"

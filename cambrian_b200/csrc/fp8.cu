@@ -16,6 +16,7 @@
 //   kv_fp8_append_kernel     cb_kv_fp8_append: the same row rule on each new K / V head row of the decode KV cache
 //   attn_decode_fp8_kernel   cb_attn_decode_fp8: flash-decoding over the FP8 cache (cambrian_b200/kv_fp8.py states it)
 #include "bytegemm.cuh"
+#include "kv_rows.cuh"
 #include <cuda_fp16.h>
 #include <algorithm>
 #include <cfloat>
@@ -447,36 +448,8 @@ int gemm_fp8_launch(const void* xq, const void* wq, const float* sa, const float
 // ---------------------------------------------------------------------------------------------------------------------
 // FP8 decode KV cache (`kv_cache_dtype="fp8"`).  Per layer kq, vq e4m3 [B, S_max, nkv, hd] and ks, vs fp32
 // [B, S_max, nkv]; each (sequence, position, kv head) row of K or V is quantised by the weight / activation rule above.
-// Both kernels give every lane KV_DPL = 8 consecutive elements of a row, so a row of hd elements is a team of hd / 8
-// adjacent lanes (16 at hd 128, 8 at hd 64) and row reductions are xor-shuffles inside the team.
+// Row helpers (one team of hd / 8 lanes per row, the row quantiser) are those of kv_rows.cuh.
 // ---------------------------------------------------------------------------------------------------------------------
-constexpr int KV_DPL = 8;
-constexpr float KV_LOG2E = 1.4426950408889634f;
-
-template <int LPK>
-__device__ __forceinline__ float team_max(float v) {
-#pragma unroll
-  for (int o = LPK / 2; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-template <int LPK>
-__device__ __forceinline__ float team_sum(float v) {
-#pragma unroll
-  for (int o = LPK / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-// 8 e4m3 (lowest byte first) -> 8 fp32, exactly: two values per packed cvt to f16x2, then f16 -> f32
-__device__ __forceinline__ void e4m3x8_to_f32(uint2 u, float* f) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const uint16_t pair = (uint16_t)(((i < 2) ? u.x : u.y) >> (16 * (i & 1)));
-    uint32_t h2;
-    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"(pair));
-    const float2 t = __half22float2(*reinterpret_cast<const __half2*>(&h2));
-    f[2 * i] = t.x;
-    f[2 * i + 1] = t.y;
-  }
-}
 
 // cb_kv_fp8_append: team r quantises row r = ((b * S + s) * nkv + h) * 2 + (0: K, 1: V) of the new tokens into position
 // offset (+ *offset_dev) + s.  No early exit: every lane of a warp takes part in the team shuffles.
@@ -508,14 +481,10 @@ __global__ void __launch_bounds__(256) kv_fp8_append_kernel(const bf16* __restri
   const long long pos = offset + (offset_dev ? *offset_dev : 0) + s;
   if (!in_range || pos < 0 || pos >= S_max) return;  // a device offset past the buffer writes nothing
   const long long cell = ((long long)b * S_max + pos) * nkv + h;
-  if (sub == 0) (which ? vs : ks)[cell] = __fdiv_rn(a, 448.0f);
-  const float rr = fminf(__fdiv_rn(448.0f, a), FLT_MAX);
-  uint32_t p[2];
-#pragma unroll
-  for (int i = 0; i < 2; ++i)
-    p[i] = f8_pack2(__fmul_rn(f[4 * i], rr), __fmul_rn(f[4 * i + 1], rr)) |
-           f8_pack2(__fmul_rn(f[4 * i + 2], rr), __fmul_rn(f[4 * i + 3], rr)) << 16;
-  *reinterpret_cast<uint2*>((which ? vq : kq) + cell * HD + sub * KV_DPL) = make_uint2(p[0], p[1]);
+  float sc;
+  const uint2 packed = kv_quant8(f, a, &sc);
+  if (sub == 0) (which ? vs : ks)[cell] = sc;
+  *reinterpret_cast<uint2*>((which ? vq : kq) + cell * HD + sub * KV_DPL) = packed;
 }
 
 // cb_attn_decode_fp8: CTA (split, kv head h, sequence b), 128 threads = TEAMS teams of LPK lanes.  The CTA owns the G

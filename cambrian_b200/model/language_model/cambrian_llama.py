@@ -27,6 +27,7 @@ except ImportError:  # pragma: no cover - older transformers
 
 from ... import ops, train_fp8
 from ...autograd import DecoderLayerFn, LinearFn, LMHeadLossFn, RMSNormFn, SpanMergeFn, SpanSplitFn
+from ...paged_kv import PagedCacheView
 from ..cambrian_arch import IGNORE_INDEX, CambrianMetaForCausalLM, CambrianMetaModel, WindowedFeatures
 
 
@@ -223,6 +224,8 @@ class CBLlamaDecoderLayer(nn.Module):
         win = {"window": self.window} if self.window else {}
         if cache is None:
             attn = ops.attn_fwd(q, k_new, v_new, causal=True, kmask=rt["kmask"], **win)
+        elif isinstance(cache, PagedCacheView):
+            attn = self._attn_paged_cache(q, k_new, v_new, cache, rt["kmask"])
         elif cache.fp8 is not None:
             attn = self._attn_fp8_cache(q, k_new, v_new, cache, rt["kmask"])
         elif cache.slot is not None:
@@ -270,6 +273,17 @@ class CBLlamaDecoderLayer(nn.Module):
         t0 = cache.length
         ops.kv_fp8_append(k_new, v_new, kq, vq, ks, vs, offset=t0)
         return ops.attn_decode_fp8(q, kq, vq, ks, vs, cache.fp8.ws, length=t0 + 1, kmask=kmask)
+
+    def _attn_paged_cache(self, q, k_new, v_new, cache, kmask):
+        """Attention with the paged cache (paged_kv.py): a prefill attends over its own bf16 K / V and is then appended
+        into its empty pages; a decode step appends each row's token at lens[b], then attends over its pages."""
+        kp, vp, ksc, vsc = cache.pool.layer(self.layer_idx)
+        if cache.prefill:
+            attn = ops.attn_fwd(q, k_new, v_new, causal=True, kmask=kmask)
+            ops.paged_kv_append(k_new, v_new, kp, vp, ksc, vsc, cache.table, offset=0)
+            return attn
+        ops.paged_kv_append(k_new, v_new, kp, vp, ksc, vsc, cache.table, cache.lens, offset_from_lens=True)
+        return ops.attn_decode_paged(q, kp, vp, ksc, vsc, cache.table, cache.lens, cache.pool.ws, len_add=1)
 
 
 class KVCache:
@@ -382,7 +396,7 @@ class CambrianLlamaModel(CambrianMetaModel, CBLlamaModel):
             inputs_embeds = EmbedSpliceFn.apply(meta, self.embed_tokens.weight, None, None)
         B, S, H = inputs_embeds.shape
         dev = inputs_embeds.device
-        cache = past_key_values if isinstance(past_key_values, KVCache) else None
+        cache = past_key_values if isinstance(past_key_values, (KVCache, PagedCacheView)) else None
         if use_cache and cache is None:
             raise ValueError("use_cache=True needs a cambrian_b200 KVCache in past_key_values (see generate())")
         past = cache.length if cache is not None else 0
@@ -579,7 +593,7 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
 
         `kv_cache_dtype` ("bf16" or "fp8", default `config.kv_cache_dtype` or "bf16") selects the decode KV cache:
         "fp8" keeps it in E4M3 with per-row scales (cambrian_b200/kv_fp8.py), about half the bytes of bf16."""
-        from ...generation import GenerationArgs, next_tokens, should_stop
+        from ...generation import next_tokens, should_stop
         from ...kv_fp8 import resolve_cache_dtype
         if "inputs_embeds" in kwargs:
             raise NotImplementedError("`inputs_embeds` is not supported")                       # :447-448
@@ -594,32 +608,12 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
         position_ids = kwargs.pop("position_ids", None)
         was_training = self.training
         self.eval()
-        feats = masks = final_size = ctx_feat = None
-        if images is not None:
-            (_, position_ids, attention_mask, _, inputs_embeds, _, feats, masks, final_size, ctx_feat) = \
-                self.prepare_inputs_labels_for_multimodal(inputs, position_ids, attention_mask, None, None, images,
-                                                          image_sizes=image_sizes)
-        else:
-            inputs_embeds = None
+        args, cache, h_last, next_pos, S0 = self._prefill(
+            inputs, images, image_sizes, attention_mask, position_ids, kwargs,
+            lambda B, S0, max_new: KVCache(self.config, B, S0 + max_new, inputs.device, dtype=kv_dtype))
         B = inputs.shape[0]
-        S0 = inputs_embeds.shape[1] if inputs_embeds is not None else inputs.shape[1]
-        args = GenerationArgs.from_kwargs(self, S0, kwargs)
         max_new = args.max_new_tokens
         dev = inputs.device
-        cache = KVCache(self.config, B, S0 + max_new, dev, dtype=kv_dtype)
-        cache.kmask = torch.ones((B, S0 + max_new), dtype=torch.bool, device=dev)
-        if attention_mask is not None:
-            cache.kmask[:, :S0] = attention_mask.bool()
-            if position_ids is None:
-                position_ids = (attention_mask.long().cumsum(1) - 1).clamp_(min=0)
-        out = self.model(input_ids=None if inputs_embeds is not None else inputs, inputs_embeds=inputs_embeds,
-                         position_ids=position_ids, past_key_values=cache, use_cache=True,
-                         vision_tower_aux_feature_list=feats, vision_tower_aux_attention_masks_list=masks,
-                         final_vision_feature_size=final_size, global_context_feature=ctx_feat)
-        last_idx = (cache.kmask[:, :S0].long().cumsum(1).argmax(1)) if attention_mask is not None else \
-            torch.full((B,), S0 - 1, device=dev)
-        h_last = out.last_hidden_state[torch.arange(B, device=dev), last_idx].contiguous()
-        next_pos = (position_ids.max(1).values + 1) if position_ids is not None else torch.full((B,), S0, device=dev)
         done = torch.zeros(B, dtype=torch.bool, device=dev)
         check_stop = bool(args.eos_token_ids or args.stopping_criteria)
         if args.streamer is not None:
@@ -651,6 +645,40 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
             args.streamer.end()
         self.train(was_training)
         return torch.stack(tokens, 1)
+
+    def _prefill(self, inputs, images, image_sizes, attention_mask, position_ids, kwargs, make_cache):
+        """The prefill of generate() and of serving.BatchedGenerator: multimodal preparation (towers, connector, splice),
+        the generation keywords (GenerationArgs, which needs the spliced prompt length S0), the cache from
+        make_cache(B, S0, max_new_tokens), the prefill forward over it, and each row's last hidden state and next
+        position.  Returns (args, cache, h_last [B, H], next_pos [B], S0)."""
+        from ...generation import GenerationArgs
+        feats = masks = final_size = ctx_feat = None
+        if images is not None:
+            (_, position_ids, attention_mask, _, inputs_embeds, _, feats, masks, final_size, ctx_feat) = \
+                self.prepare_inputs_labels_for_multimodal(inputs, position_ids, attention_mask, None, None, images,
+                                                          image_sizes=image_sizes)
+        else:
+            inputs_embeds = None
+        B = inputs.shape[0]
+        S0 = inputs_embeds.shape[1] if inputs_embeds is not None else inputs.shape[1]
+        args = GenerationArgs.from_kwargs(self, S0, kwargs)
+        max_new = args.max_new_tokens
+        dev = inputs.device
+        cache = make_cache(B, S0, max_new)
+        cache.kmask = torch.ones((B, S0 + max_new), dtype=torch.bool, device=dev)
+        if attention_mask is not None:
+            cache.kmask[:, :S0] = attention_mask.bool()
+            if position_ids is None:
+                position_ids = (attention_mask.long().cumsum(1) - 1).clamp_(min=0)
+        out = self.model(input_ids=None if inputs_embeds is not None else inputs, inputs_embeds=inputs_embeds,
+                         position_ids=position_ids, past_key_values=cache, use_cache=True,
+                         vision_tower_aux_feature_list=feats, vision_tower_aux_attention_masks_list=masks,
+                         final_vision_feature_size=final_size, global_context_feature=ctx_feat)
+        last_idx = (cache.kmask[:, :S0].long().cumsum(1).argmax(1)) if attention_mask is not None else \
+            torch.full((B,), S0 - 1, device=dev)
+        h_last = out.last_hidden_state[torch.arange(B, device=dev), last_idx].contiguous()
+        next_pos = (position_ids.max(1).values + 1) if position_ids is not None else torch.full((B,), S0, device=dev)
+        return args, cache, h_last, next_pos, S0
 
     def _generate_graphed(self, args, cache, h_last, next_pos, S0, max_new, check_stop):
         """Greedy decoding with ONE CUDA graph per generate() call: a decode step is ~290 kernel launches whose device time

@@ -1100,3 +1100,86 @@ def attn_decode_fp8(q, kq, vq, ks, vs, workspace, *, length: int, length_dev=Non
                                          ptr(workspace), workspace.numel(), B, Sq, nh, nkv, S_max, hd, int(length),
                                          ptr(length_dev), float(scale), stream()), "cb_attn_decode_fp8")
     return o
+
+
+# ------------------------------------------------------------------------------------------------
+# Paged decode KV cache (serving.BatchedGenerator; the format lives in paged_kv.py)
+# ------------------------------------------------------------------------------------------------
+def _paged_pages(what, kp, vp, ksc, vsc, hd=None):
+    """(fp8, num_pages, page_size, nkv, hd) of one layer's pages, after checking dtypes and shapes."""
+    if kp.dim() != 4 or vp.shape != kp.shape or vp.dtype != kp.dtype or not (kp.is_contiguous() and vp.is_contiguous()):
+        raise ValueError(f"{what}: k / v pages must be contiguous [num_pages, page_size, nkv, hd] of one dtype")
+    fp8 = kp.dtype == torch.float8_e4m3fn
+    if not fp8 and kp.dtype != torch.bfloat16:
+        raise ValueError(f"{what}: pages must be bf16 or float8_e4m3fn, not {kp.dtype}")
+    if fp8 and (ksc is None or vsc is None or ksc.shape != kp.shape[:3] or vsc.shape != ksc.shape
+                or ksc.dtype != torch.float32 or vsc.dtype != torch.float32
+                or not (ksc.is_contiguous() and vsc.is_contiguous())):
+        raise ValueError(f"{what}: FP8 pages need contiguous fp32 scales [num_pages, page_size, nkv]")
+    if not fp8 and (ksc is not None or vsc is not None):
+        raise ValueError(f"{what}: bf16 pages take no scales")
+    num_pages, page_size, nkv, phd = kp.shape
+    if hd is not None and phd != hd:
+        raise ValueError(f"{what}: pages hold head_dim {phd}, the rows {hd}")
+    return int(fp8), num_pages, page_size, nkv, phd
+
+
+def _paged_table(what, table, lens, rows, need_lens):
+    if table.dim() != 2 or table.dtype != torch.int32 or table.shape[0] != rows or table.stride(1) != 1:
+        raise ValueError(f"{what}: block_table must be int32 [rows={rows}, max_pages] with contiguous rows")
+    if lens is None:
+        if need_lens:
+            raise ValueError(f"{what}: lens is required")
+    elif lens.dtype != torch.int32 or lens.shape != (rows,) or not lens.is_contiguous():
+        raise ValueError(f"{what}: lens must be a contiguous int32 [rows={rows}]")
+    return table.shape[1], (table.stride(0) if rows > 1 else table.shape[1])
+
+
+def paged_kv_append(k, v, k_pages, v_pages, k_scales, v_scales, block_table, lens=None, offset: int = 0,
+                    offset_from_lens: bool = False):
+    """Write the new rows k, v [rows, S, nkv, hd] (views of the packed post-RoPE qkv rows, read in place) into one
+    layer's pages at positions offset (+ lens[b] with offset_from_lens) + s through block_table; a row with lens[b] < 0
+    writes nothing."""
+    _require_cuda_bf16(k, v)
+    B, S, nkv, hd = k.shape
+    ld = k.stride(1) if S > 1 else (k.stride(0) if B > 1 else nkv * hd)
+    if (v.shape != k.shape or v.stride() != k.stride() or k.stride(3) != 1 or (nkv > 1 and k.stride(2) != hd)
+            or (B > 1 and k.stride(0) != S * ld)):
+        raise ValueError(f"paged_kv_append: k, v must be [rows, S, nkv, hd] rows at one common stride, got {k.stride()}")
+    fp8, num_pages, page_size, pnkv, _ = _paged_pages("paged_kv_append", k_pages, v_pages, k_scales, v_scales, hd)
+    if pnkv != nkv:
+        raise ValueError(f"paged_kv_append: pages hold {pnkv} kv heads, the rows {nkv}")
+    max_pages, tld = _paged_table("paged_kv_append", block_table, lens, B, offset_from_lens)
+    check(_lib.load().cb_paged_kv_append(ptr(k), ptr(v), ld, ptr(k_pages), ptr(v_pages), ptr(k_scales), ptr(v_scales),
+                                         fp8, ptr(block_table), tld, ptr(lens), B, S, nkv, hd, page_size, num_pages,
+                                         max_pages, int(offset), int(bool(offset_from_lens)), stream()),
+          "cb_paged_kv_append")
+
+
+def attn_decode_paged_workspace(rows: int, nh: int, max_pages: int, page_size: int, hd: int, device) -> torch.Tensor:
+    """The fp32 workspace `attn_decode_paged` needs for up to `rows` rows (at least one element)."""
+    n = _lib.load().cb_attn_decode_paged_workspace_floats(rows, nh, max_pages, page_size, hd)
+    return torch.empty(max(int(n), 1), dtype=torch.float32, device=device)
+
+
+def attn_decode_paged(q, k_pages, v_pages, k_scales, v_scales, block_table, lens, workspace, *, len_add: int = 1,
+                      scale: float | None = None):
+    """Decode attention over one layer's pages: q [rows, 1, nh, hd] (a view of the packed qkv row) -> o [rows, 1, nh, hd]
+    bf16.  Row b attends over its positions below lens[b] + len_add; a row with lens[b] < 0 gets zeros."""
+    _require_cuda_bf16(q)
+    B, Sq, nh, hd = q.shape
+    if Sq != 1:
+        raise ValueError(f"attn_decode_paged: Sq={Sq}; the paged decode kernel takes one query per row")
+    if scale is None:
+        scale = hd ** -0.5
+    qb, _ = _bshd_strides(q, hd)
+    fp8, num_pages, page_size, nkv, _ = _paged_pages("attn_decode_paged", k_pages, v_pages, k_scales, v_scales, hd)
+    max_pages, tld = _paged_table("attn_decode_paged", block_table, lens, B, True)
+    if workspace.dtype != torch.float32:
+        raise ValueError("attn_decode_paged: the workspace must be fp32")
+    o = torch.empty((B, 1, nh, hd), dtype=torch.bfloat16, device=q.device)
+    check(_lib.load().cb_attn_decode_paged(ptr(q), qb, ptr(k_pages), ptr(v_pages), ptr(k_scales), ptr(v_scales), fp8,
+                                           ptr(block_table), tld, ptr(lens), int(len_add), ptr(o), ptr(workspace),
+                                           workspace.numel(), B, nh, nkv, hd, page_size, num_pages, max_pages,
+                                           float(scale), stream()), "cb_attn_decode_paged")
+    return o

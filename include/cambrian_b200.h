@@ -404,6 +404,38 @@ int cb_rmsnorm_fwd_fp8(const void* x, const void* gamma, void* xq, float* sa, fl
  * row: bit for bit cb_fp8_quantize_act of the [rows, 2I] gradient.  I % 8 == 0; one CTA per row, no atomics. */
 int cb_swiglu_bwd_fp8(const void* dout, const void* gate, const void* up, void* dgate, void* dup, void* dguq, float* sdgu,
                       int64_t rows, int I, int64_t ld_in, int64_t ld_dout, int64_t ld_dgu, void* stream);
+/* Paged decode KV cache for continuous batching (cambrian_b200/serving.py; the format is defined in
+ * cambrian_b200/paged_kv.py).  The reference serves many requests at once through SGLang (serve/sglang_worker.py) and
+ * keeps HF's per-call cache behind LlamaSdpaAttention (the cache update and decode-step SDPA of cambrian_llama.py:437-483
+ * through GenerationMixin.generate); these replace that cache update and decode SDPA for a batch of independent
+ * sequences.  Per layer K and V pages [num_pages, page_size, nkv, hd] (position-major inside a page), bf16 (fp8 == 0) or
+ * e4m3 with fp32 scales [num_pages, page_size, nkv] by the row rule of cb_kv_fp8_append (fp8 == 1).  block_table int32
+ * [rows, table_ld]: entry (b, p) is the page holding positions [p * page_size, (p + 1) * page_size) of row b (only the
+ * first max_pages columns are read).  lens int32 [rows]: row b's cached length; a negative length marks an inactive
+ * (padding) row.  page_size is a power of two >= 16; hd 64 or 128.  A table entry outside [0, num_pages) is skipped.
+ *
+ * cb_paged_kv_append: the new rows k, v (element (b, s, h, d) at base + (b * S + s) * ld + h * hd + d: the K and V heads
+ * of the packed post-RoPE qkv rows, read in place) go to position offset + s, plus lens[b] when offset_from_lens (the
+ * graph-replayed decode step).  lens may be NULL when !offset_from_lens; an inactive row writes nothing.  FP8 pages get
+ * bit for bit the bytes and scales cb_kv_fp8_append writes for the same rows. */
+int cb_paged_kv_append(const void* k, const void* v, int64_t ld, void* k_pages, void* v_pages, float* k_scales,
+                       float* v_scales, int fp8, const int* block_table, int64_t table_ld, const int* lens, int rows, int S,
+                       int nkv, int hd, int page_size, int num_pages, int max_pages, int64_t offset, int offset_from_lens,
+                       void* stream);
+/* fp32 workspace cb_attn_decode_paged needs: rows * nh * ceil(max_pages * page_size / 256) * (hd + 2) */
+int64_t cb_attn_decode_paged_workspace_floats(int rows, int nh, int max_pages, int page_size, int hd);
+/* Decode attention over the pages (flash-decoding), one query per row: q element (b, h, d) at q + b * q_bs + h * hd + d
+ * (a view of the packed qkv row), o [rows, nh, hd] bf16 contiguous.  Valid keys of row b: positions below
+ * lens[b] + len_add (len_add = 1 counts the row appended just before).  One CTA per (key split, kv head, row) serves the
+ * nh / nkv (1..8) query heads of that kv head, so each cached byte is read once per call, and only below the valid
+ * length.  Every split covers 256 key positions, independent of rows, bucket and SM count; the grid is sized from
+ * max_pages and splits past a row's length exit.  Partials are merged in split order through `workspace` (no atomics),
+ * so a row's output is bitwise independent of the other rows of the launch.  bf16 pages: scores and the PV sum in fp32,
+ * one rounding to bf16; FP8 pages: the decode arithmetic of cb_attn_decode_fp8.  A row of length <= 0 gets zeros. */
+int cb_attn_decode_paged(const void* q, int64_t q_bs, const void* k_pages, const void* v_pages, const float* k_scales,
+                         const float* v_scales, int fp8, const int* block_table, int64_t table_ld, const int* lens,
+                         int len_add, void* o, float* workspace, int64_t workspace_floats, int rows, int nh, int nkv, int hd,
+                         int page_size, int num_pages, int max_pages, float scale, void* stream);
 
 #ifdef __cplusplus
 }
