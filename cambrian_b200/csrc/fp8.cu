@@ -13,10 +13,7 @@
 //   f8_quant_rows_kernel     cb_fp8_quantize_weight / cb_fp8_quantize_act: one CTA per row, amax then q; no atomics
 //   gemm_fp8_wgmma           M > 8 (cb_gemm_fp8): bytegemm.cuh's TMA ring, wgmma m64n128k32 .f32.e4m3.e4m3
 //   gemv_fp8_wgmma           M <= 8 (cb_gemv_fp8): swap AB, y^T = W x^T as wgmma m64n8k32, K split over a cluster
-//   kv_fp8_append_kernel     cb_kv_fp8_append: the same row rule on each new K / V head row of the decode KV cache
-//   attn_decode_fp8_kernel   cb_attn_decode_fp8: flash-decoding over the FP8 cache (cambrian_b200/kv_fp8.py states it)
 #include "bytegemm.cuh"
-#include "kv_rows.cuh"
 #include <cuda_fp16.h>
 #include <algorithm>
 #include <cfloat>
@@ -442,332 +439,6 @@ int gemm_fp8_launch(const void* xq, const void* wq, const float* sa, const float
   const unsigned grid = (unsigned)std::min<long long>(tiles, device_sm_count());
   gemm_fp8_wgmma<<<grid, 288, F8_SMEM_BYTES, st>>>(ta, tb, tc, M, N, K, (int)tiles, tma_store, ep);
   CB_CUDA_LAUNCH_CHECK("gemm_fp8_wgmma");
-  return CB_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// FP8 decode KV cache (`kv_cache_dtype="fp8"`).  Per layer kq, vq e4m3 [B, S_max, nkv, hd] and ks, vs fp32
-// [B, S_max, nkv]; each (sequence, position, kv head) row of K or V is quantised by the weight / activation rule above.
-// Row helpers (one team of hd / 8 lanes per row, the row quantiser) are those of kv_rows.cuh.
-// ---------------------------------------------------------------------------------------------------------------------
-
-// cb_kv_fp8_append: team r quantises row r = ((b * S + s) * nkv + h) * 2 + (0: K, 1: V) of the new tokens into position
-// offset (+ *offset_dev) + s.  No early exit: every lane of a warp takes part in the team shuffles.
-template <int HD>
-__global__ void __launch_bounds__(256) kv_fp8_append_kernel(const bf16* __restrict__ k, const bf16* __restrict__ v,
-                                                            long long ld, uint8_t* __restrict__ kq, uint8_t* __restrict__ vq,
-                                                            float* __restrict__ ks, float* __restrict__ vs, int B, int S,
-                                                            int S_max, int nkv, long long offset,
-                                                            const long long* __restrict__ offset_dev) {
-  constexpr int LPK = HD / KV_DPL;
-  const long long rows = 2LL * B * S * nkv;
-  const long long r0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / LPK;
-  const int sub = threadIdx.x % LPK;
-  const bool in_range = r0 < rows;
-  const long long r = in_range ? r0 : 0;
-  const int which = (int)(r & 1);
-  long long t = r >> 1;
-  const int h = (int)(t % nkv);
-  t /= nkv;
-  const int s = (int)(t % S);
-  const int b = (int)(t / S);
-  const bf16* src = (which ? v : k) + ((long long)b * S + s) * ld + h * HD + sub * KV_DPL;
-  float f[8];
-  unpack8(*reinterpret_cast<const uint4*>(src), f);
-  float a = 0.f;
-#pragma unroll
-  for (int e = 0; e < 8; ++e) a = fmaxf(a, fabsf(f[e]));
-  a = team_max<LPK>(a);
-  const long long pos = offset + (offset_dev ? *offset_dev : 0) + s;
-  if (!in_range || pos < 0 || pos >= S_max) return;  // a device offset past the buffer writes nothing
-  const long long cell = ((long long)b * S_max + pos) * nkv + h;
-  float sc;
-  const uint2 packed = kv_quant8(f, a, &sc);
-  if (sub == 0) (which ? vs : ks)[cell] = sc;
-  *reinterpret_cast<uint2*>((which ? vq : kq) + cell * HD + sub * KV_DPL) = packed;
-}
-
-// cb_attn_decode_fp8: CTA (split, kv head h, sequence b), 128 threads = TEAMS teams of LPK lanes.  The CTA owns the G
-// query heads of kv head h and the key chunk [split * chunk, +chunk) clipped to the valid length L; a chunk wholly past L
-// returns before it reads anything.  Each team walks its keys (team, team + TEAMS, ...) BLK at a time: per key one
-// 8-byte load of K and of V per lane, G dot products of 8 elements from registers, a team sum, then per head
-// score = (dot * ks) * scale and an online softmax in fp32 (one rescale per BLK keys); o += (p * vs) * float(vq).  Keys
-// past L or masked out are never loaded.  The teams' (m, l, o) states are merged in team order through shared memory;
-// with one split the CTA normalises and stores, otherwise it writes its (m, l, o) to the workspace for
-// attn_decode_fp8_combine, which merges the splits in split order.  Fixed orders throughout: bitwise run to run.
-constexpr int KVD_THREADS = 128;
-constexpr int KVD_MIN_CHUNK = 256;  // keys a split owns at least
-constexpr int KVD_MAX_SPLITS = 64;
-
-template <int HD, int G>
-__global__ void __launch_bounds__(KVD_THREADS)
-attn_decode_fp8_kernel(const bf16* __restrict__ q, long long q_bs, const uint8_t* __restrict__ kq,
-                       const uint8_t* __restrict__ vq, const float* __restrict__ ks, const float* __restrict__ vs,
-                       const uint8_t* __restrict__ kmask, long long kmask_ld, bf16* __restrict__ o,
-                       float* __restrict__ ws, int nkv, int S_max, int chunk, int nsplit, long long length,
-                       const long long* __restrict__ length_dev, float scale) {
-  constexpr int LPK = HD / KV_DPL;
-  constexpr int TEAMS = KVD_THREADS / LPK;
-  constexpr int BLK = G <= 4 ? 4 : 2;
-  constexpr int ST = HD + 2;  // per-head state: m, l, o[HD]
-  __shared__ float red[TEAMS][G][ST];
-  const int split = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-  const int nh = nkv * G;
-  long long L = length + (length_dev ? *length_dev : 0);
-  L = L < (long long)S_max ? L : (long long)S_max;
-  const int t0 = split * chunk;
-  if (split > 0 && t0 >= L) return;  // split 0 always runs, so an empty cache still yields a defined (zero) output
-  const int t1 = (int)(t0 + chunk < L ? t0 + chunk : L);
-  const int team = threadIdx.x / LPK, sub = threadIdx.x % LPK;
-
-  float qf[G][8];
-#pragma unroll
-  for (int g = 0; g < G; ++g)
-    unpack8(*reinterpret_cast<const uint4*>(q + (long long)b * q_bs + (h * G + g) * HD + sub * KV_DPL), qf[g]);
-  const long long row = (long long)nkv * HD;  // bytes from one position to the next
-  const uint8_t* kb = kq + ((long long)b * S_max * nkv + h) * HD + sub * KV_DPL;
-  const uint8_t* vb = vq + ((long long)b * S_max * nkv + h) * HD + sub * KV_DPL;
-  const float* ksb = ks + (long long)b * S_max * nkv + h;
-  const float* vsb = vs + (long long)b * S_max * nkv + h;
-  const uint8_t* mb = kmask ? kmask + (long long)b * kmask_ld : nullptr;
-
-  float m[G], l[G], acc[G][8];
-#pragma unroll
-  for (int g = 0; g < G; ++g) {
-    m[g] = -INFINITY;
-    l[g] = 0.f;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) acc[g][e] = 0.f;
-  }
-  // the trip count is the same for every team (t0, t1 are per CTA), so the team shuffles never diverge
-  for (int base = t0; base < t1; base += TEAMS * BLK) {
-    uint2 kr[BLK], vr[BLK];
-    float ksv[BLK], vsv[BLK];
-    unsigned okm = 0u;  // bit j: key j of the block is valid
-#pragma unroll
-    for (int j = 0; j < BLK; ++j) {
-      const int t = base + team + j * TEAMS;
-      const bool valid = t < t1 && (!mb || mb[t]);
-      okm |= valid ? 1u << j : 0u;
-      kr[j] = vr[j] = make_uint2(0u, 0u);
-      ksv[j] = vsv[j] = 0.f;
-      if (valid) {
-        kr[j] = *reinterpret_cast<const uint2*>(kb + t * row);
-        vr[j] = *reinterpret_cast<const uint2*>(vb + t * row);
-        ksv[j] = ksb[(long long)t * nkv];
-        vsv[j] = vsb[(long long)t * nkv];
-      }
-    }
-    float s[BLK][G];
-#pragma unroll
-    for (int j = 0; j < BLK; ++j) {
-      float kf[8];
-      e4m3x8_to_f32(kr[j], kf);
-#pragma unroll
-      for (int g = 0; g < G; ++g) {
-        float d = 0.f;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) d = fmaf(qf[g][e], kf[e], d);
-        d = team_sum<LPK>(d);
-        s[j][g] = (okm >> j) & 1u ? __fmul_rn(__fmul_rn(d, ksv[j]), scale) : -INFINITY;
-      }
-    }
-    float pv[BLK][G];
-#pragma unroll
-    for (int g = 0; g < G; ++g) {
-      float mx = m[g];
-#pragma unroll
-      for (int j = 0; j < BLK; ++j) mx = fmaxf(mx, s[j][g]);
-      const float c = m[g] == -INFINITY ? 0.f : fast_exp2((m[g] - mx) * KV_LOG2E);
-      float ls = __fmul_rn(l[g], c);
-#pragma unroll
-      for (int j = 0; j < BLK; ++j) {
-        const float p = (okm >> j) & 1u ? fast_exp2((s[j][g] - mx) * KV_LOG2E) : 0.f;
-        ls += p;
-        pv[j][g] = __fmul_rn(p, vsv[j]);
-      }
-      l[g] = ls;
-      m[g] = mx;
-#pragma unroll
-      for (int e = 0; e < 8; ++e) acc[g][e] = __fmul_rn(acc[g][e], c);
-    }
-#pragma unroll
-    for (int j = 0; j < BLK; ++j) {
-      float vf[8];
-      e4m3x8_to_f32(vr[j], vf);
-#pragma unroll
-      for (int g = 0; g < G; ++g)
-#pragma unroll
-        for (int e = 0; e < 8; ++e) acc[g][e] = fmaf(pv[j][g], vf[e], acc[g][e]);
-    }
-  }
-
-#pragma unroll
-  for (int g = 0; g < G; ++g) {
-    if (sub == 0) {
-      red[team][g][0] = m[g];
-      red[team][g][1] = l[g];
-    }
-#pragma unroll
-    for (int e = 0; e < 8; ++e) red[team][g][2 + sub * KV_DPL + e] = acc[g][e];
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < G * HD; i += KVD_THREADS) {
-    const int g = i / HD, d = i % HD;
-    float M = -INFINITY;
-#pragma unroll
-    for (int tm = 0; tm < TEAMS; ++tm) M = fmaxf(M, red[tm][g][0]);
-    float Ls = 0.f, Os = 0.f;
-    if (M != -INFINITY) {
-#pragma unroll
-      for (int tm = 0; tm < TEAMS; ++tm) {
-        const float mt = red[tm][g][0];
-        const float w = mt == -INFINITY ? 0.f : fast_exp2((mt - M) * KV_LOG2E);
-        Ls = fmaf(red[tm][g][1], w, Ls);
-        Os = fmaf(red[tm][g][2 + d], w, Os);
-      }
-    }
-    const long long bh = (long long)b * nh + h * G + g;
-    if (nsplit == 1) {
-      o[bh * HD + d] = __float2bfloat16(Ls > 0.f ? __fdiv_rn(Os, Ls) : 0.f);
-    } else {
-      float* w = ws + (bh * nsplit + split) * ST;
-      if (d == 0) {
-        w[0] = M;
-        w[1] = Ls;
-      }
-      w[2 + d] = Os;
-    }
-  }
-}
-
-// one CTA per (sequence, query head), thread d: the splits that hold valid keys, merged in split order
-template <int HD>
-__global__ void __launch_bounds__(HD) attn_decode_fp8_combine(const float* __restrict__ ws, bf16* __restrict__ o, int S_max,
-                                                              int chunk, int nsplit, long long length,
-                                                              const long long* __restrict__ length_dev) {
-  constexpr int ST = HD + 2;
-  long long L = length + (length_dev ? *length_dev : 0);
-  L = L < (long long)S_max ? L : (long long)S_max;
-  const int active = L <= 0 ? 0 : (int)((L + chunk - 1) / chunk);
-  const long long bh = blockIdx.x;
-  const int d = threadIdx.x;
-  const float* w = ws + bh * nsplit * ST;
-  float M = -INFINITY;
-  for (int sp = 0; sp < active; ++sp) M = fmaxf(M, w[sp * ST]);
-  float Ls = 0.f, Os = 0.f;
-  if (M != -INFINITY) {
-    for (int sp = 0; sp < active; ++sp) {
-      const float ms = w[sp * ST];
-      const float e = ms == -INFINITY ? 0.f : fast_exp2((ms - M) * KV_LOG2E);
-      Ls = fmaf(w[sp * ST + 1], e, Ls);
-      Os = fmaf(w[sp * ST + 2 + d], e, Os);
-    }
-  }
-  o[bh * HD + d] = __float2bfloat16(Ls > 0.f ? __fdiv_rn(Os, Ls) : 0.f);
-}
-
-int kv_fp8_append_launch(const void* k, const void* v, long long ld, void* kq, void* vq, float* ks, float* vs, int B, int S,
-                         int S_max, int nkv, int hd, long long offset, const long long* offset_dev, cudaStream_t st) {
-  CB_CHECK_ARG(hd == 64 || hd == 128, "kv_fp8_append: hd=%d must be 64 or 128", hd);
-  CB_CHECK_ARG(B > 0 && S > 0 && S_max > 0 && nkv > 0, "kv_fp8_append: empty problem (B=%d S=%d S_max=%d nkv=%d)", B, S,
-               S_max, nkv);
-  CB_CHECK_ARG(k && v && kq && vq && ks && vs, "kv_fp8_append: null argument");
-  CB_CHECK_ARG(ld >= (long long)nkv * hd && ld % 8 == 0, "kv_fp8_append: row stride %lld must be >= nkv*hd and a multiple of 8",
-               ld);
-  CB_CHECK_ARG(((reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v)) & 15u) == 0 &&
-                   ((reinterpret_cast<uintptr_t>(kq) | reinterpret_cast<uintptr_t>(vq)) & 7u) == 0 &&
-                   ((reinterpret_cast<uintptr_t>(ks) | reinterpret_cast<uintptr_t>(vs)) & 3u) == 0,
-               "kv_fp8_append: k, v must be 16-byte aligned, kq, vq 8-byte aligned");
-  CB_CHECK_ARG(offset >= 0 && (offset_dev || offset + S <= S_max), "kv_fp8_append: positions [%lld, %lld) outside the cache (%d)",
-               offset, offset + S, S_max);
-  const long long threads = 2LL * B * S * nkv * (hd / KV_DPL);
-  const long long blocks = (threads + 255) / 256;
-  CB_CHECK_ARG(blocks < (1LL << 31), "kv_fp8_append: too many rows");
-  if (hd == 128)
-    kv_fp8_append_kernel<128><<<(unsigned)blocks, 256, 0, st>>>((const bf16*)k, (const bf16*)v, ld, (uint8_t*)kq,
-                                                                (uint8_t*)vq, ks, vs, B, S, S_max, nkv, offset, offset_dev);
-  else
-    kv_fp8_append_kernel<64><<<(unsigned)blocks, 256, 0, st>>>((const bf16*)k, (const bf16*)v, ld, (uint8_t*)kq,
-                                                               (uint8_t*)vq, ks, vs, B, S, S_max, nkv, offset, offset_dev);
-  CB_CUDA_LAUNCH_CHECK("kv_fp8_append_kernel");
-  return CB_OK;
-}
-
-// the split count: enough CTAs for about three per SM over (B, nkv), each split at least KVD_MIN_CHUNK keys of S_max
-static int kvd_splits(int B, int nkv, int S_max, int* chunk) {
-  const long long bk = (long long)B * nkv;
-  const long long want = (3LL * device_sm_count() + bk - 1) / bk;
-  const long long by_len = (S_max + KVD_MIN_CHUNK - 1) / KVD_MIN_CHUNK;
-  int n = (int)std::max(1LL, std::min({want, by_len, (long long)KVD_MAX_SPLITS}));
-  *chunk = (S_max + n - 1) / n;
-  return (S_max + *chunk - 1) / *chunk;
-}
-
-long long attn_decode_fp8_workspace_floats(int B, int nh, int nkv, int S_max, int hd) {
-  if (B <= 0 || nh <= 0 || nkv <= 0 || S_max <= 0 || hd <= 0) return 0;
-  int chunk;
-  const int n = kvd_splits(B, nkv, S_max, &chunk);
-  return n > 1 ? (long long)B * nh * n * (hd + 2) : 0;
-}
-
-template <int HD>
-static void kvd_launch(int G, dim3 grid, cudaStream_t st, const bf16* q, long long q_bs, const uint8_t* kq,
-                       const uint8_t* vq, const float* ks, const float* vs, const uint8_t* km, long long km_ld, bf16* o,
-                       float* ws, int nkv, int S_max, int chunk, int nsplit, long long length, const long long* length_dev,
-                       float scale) {
-#define KVD_CASE(GG)                                                                                                     \
-  case GG:                                                                                                               \
-    attn_decode_fp8_kernel<HD, GG><<<grid, KVD_THREADS, 0, st>>>(q, q_bs, kq, vq, ks, vs, km, km_ld, o, ws, nkv, S_max, \
-                                                                 chunk, nsplit, length, length_dev, scale);              \
-    break;
-  switch (G) {
-    KVD_CASE(1) KVD_CASE(2) KVD_CASE(3) KVD_CASE(4) KVD_CASE(5) KVD_CASE(6) KVD_CASE(7) KVD_CASE(8)
-  }
-#undef KVD_CASE
-}
-
-int attn_decode_fp8_launch(const void* q, long long q_bs, const void* kq, const void* vq, const float* ks, const float* vs,
-                           const void* kmask, long long kmask_ld, void* o, float* ws, long long ws_floats, int B, int Sq,
-                           int nh, int nkv, int S_max, int hd, long long length, const long long* length_dev, float scale,
-                           cudaStream_t st) {
-  CB_CHECK_ARG(Sq == 1, "attn_decode_fp8: Sq=%d; the decode kernel takes one query per sequence", Sq);
-  CB_CHECK_ARG(hd == 64 || hd == 128, "attn_decode_fp8: hd=%d must be 64 or 128", hd);
-  CB_CHECK_ARG(B > 0 && B < 65536 && nkv > 0 && nkv < 65536 && S_max > 0, "attn_decode_fp8: bad shape (B=%d nkv=%d S_max=%d)",
-               B, nkv, S_max);
-  CB_CHECK_ARG(nh % nkv == 0 && nh / nkv >= 1 && nh / nkv <= 8,
-               "attn_decode_fp8: nh=%d must be 1..8 times nkv=%d (query heads per kv head)", nh, nkv);
-  CB_CHECK_ARG(q && kq && vq && ks && vs && o, "attn_decode_fp8: null argument");
-  CB_CHECK_ARG(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(o)) & 15u) == 0 && q_bs % 8 == 0 &&
-                   q_bs >= (long long)nh * hd && ((reinterpret_cast<uintptr_t>(kq) | reinterpret_cast<uintptr_t>(vq)) & 7u) == 0 &&
-                   ((reinterpret_cast<uintptr_t>(ks) | reinterpret_cast<uintptr_t>(vs)) & 3u) == 0,
-               "attn_decode_fp8: q, o must be 16-byte aligned (q batch stride a multiple of 8), kq, vq 8-byte aligned");
-  CB_CHECK_ARG(length >= 0 && (length_dev || length <= S_max), "attn_decode_fp8: length %lld outside the cache (%d)", length,
-               S_max);
-  CB_CHECK_ARG(!kmask || kmask_ld >= (length_dev ? (long long)S_max : length),
-               "attn_decode_fp8: kmask row stride %lld does not cover the valid keys", kmask_ld);
-  int chunk;
-  const int nsplit = kvd_splits(B, nkv, S_max, &chunk);
-  if (nsplit > 1) {
-    const long long need = (long long)B * nh * nsplit * (hd + 2);
-    CB_CHECK_ARG(ws && ws_floats >= need, "attn_decode_fp8: workspace of %lld floats, %lld needed", ws_floats, need);
-  }
-  const int G = nh / nkv;
-  const dim3 grid(nsplit, nkv, B);
-  if (hd == 128)
-    kvd_launch<128>(G, grid, st, (const bf16*)q, q_bs, (const uint8_t*)kq, (const uint8_t*)vq, ks, vs, (const uint8_t*)kmask,
-                    kmask_ld, (bf16*)o, ws, nkv, S_max, chunk, nsplit, length, length_dev, scale);
-  else
-    kvd_launch<64>(G, grid, st, (const bf16*)q, q_bs, (const uint8_t*)kq, (const uint8_t*)vq, ks, vs, (const uint8_t*)kmask,
-                   kmask_ld, (bf16*)o, ws, nkv, S_max, chunk, nsplit, length, length_dev, scale);
-  CB_CUDA_LAUNCH_CHECK("attn_decode_fp8_kernel");
-  if (nsplit > 1) {
-    if (hd == 128)
-      attn_decode_fp8_combine<128><<<B * nh, 128, 0, st>>>(ws, (bf16*)o, S_max, chunk, nsplit, length, length_dev);
-    else
-      attn_decode_fp8_combine<64><<<B * nh, 64, 0, st>>>(ws, (bf16*)o, S_max, chunk, nsplit, length, length_dev);
-    CB_CUDA_LAUNCH_CHECK("attn_decode_fp8_combine");
-  }
   return CB_OK;
 }
 

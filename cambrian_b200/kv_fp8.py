@@ -1,7 +1,8 @@
 """FP8 E4M3 decode KV cache (`generate(..., kv_cache_dtype="fp8")`).
 
-This module is the one place on the host that states the format and its arithmetic (the kernels `kv_fp8_append_kernel`
-and `attn_decode_fp8_kernel` in csrc/fp8.cu are the other side).  E4M3 and e4m3_rn_satfinite are those of quant_fp8.py.
+This module is the one place on the host that states the format and its arithmetic (the kernels `kv_append_kernel` and
+`kv_decode_kernel` over `DenseCells` in csrc/kv_cache.cu are the other side; the paged cache of paged_kv.py runs the same
+kernels over `PagedCells`).  E4M3 and e4m3_rn_satfinite are those of quant_fp8.py.
 
 Rows.  Each cached row is the hd elements of one (sequence, position, kv head) of K or of V, after RoPE, as the decoder
 layer's packed qkv GEMM output holds them (bf16).  K and V are separate rows.

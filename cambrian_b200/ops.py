@@ -1038,19 +1038,28 @@ def swiglu_bwd_fp8(dout, gate, up, dgate, dup):
 
 
 # ------------------------------------------------------------------------------------------------
-# FP8 E4M3 decode KV cache (kv_cache_dtype="fp8"; the format and the decode arithmetic live in kv_fp8.py)
+# Decode KV caches: the dense FP8 cache (kv_cache_dtype="fp8"; the format and the decode arithmetic live in kv_fp8.py)
+# and the paged cache (serving.BatchedGenerator; the format lives in paged_kv.py)
 # ------------------------------------------------------------------------------------------------
-def kv_fp8_append(k, v, kq, vq, ks, vs, offset: int = 0, offset_dev=None):
-    """Quantise the new rows k, v [B, S, nkv, hd] (views of the packed post-RoPE qkv rows, read in place) into one
-    layer's FP8 cache kq, vq [B, S_max, nkv, hd] float8_e4m3fn, ks, vs [B, S_max, nkv] fp32 at positions offset + s
-    (+ offset_dev[0], a device int64, for the graph-replayed step)."""
+def _kv_new_rows(what, k, v, rows="B") -> int:
+    """The row stride of the new K / V rows k, v [rows, S, nkv, hd] an append reads in place, after checking them;
+    `rows` names the first dimension in the error message."""
     _require_cuda_bf16(k, v)
     B, S, nkv, hd = k.shape
     # the row stride: a size-1 dimension's stride says nothing, so one token per sequence takes it from the batch stride
     ld = k.stride(1) if S > 1 else (k.stride(0) if B > 1 else nkv * hd)
     if (v.shape != k.shape or v.stride() != k.stride() or k.stride(3) != 1 or (nkv > 1 and k.stride(2) != hd)
             or (B > 1 and k.stride(0) != S * ld)):
-        raise ValueError(f"kv_fp8_append: k, v must be [B, S, nkv, hd] rows at one common stride, got {k.stride()}")
+        raise ValueError(f"{what}: k, v must be [{rows}, S, nkv, hd] rows at one common stride, got {k.stride()}")
+    return ld
+
+
+def kv_fp8_append(k, v, kq, vq, ks, vs, offset: int = 0, offset_dev=None):
+    """Quantise the new rows k, v [B, S, nkv, hd] (views of the packed post-RoPE qkv rows, read in place) into one
+    layer's FP8 cache kq, vq [B, S_max, nkv, hd] float8_e4m3fn, ks, vs [B, S_max, nkv] fp32 at positions offset + s
+    (+ offset_dev[0], a device int64, for the graph-replayed step)."""
+    ld = _kv_new_rows("kv_fp8_append", k, v)
+    B, S, nkv, hd = k.shape
     S_max = kq.shape[1]
     if (kq.shape != (B, S_max, nkv, hd) or vq.shape != kq.shape or kq.dtype != torch.float8_e4m3fn
             or vq.dtype != kq.dtype or ks.shape != (B, S_max, nkv) or vs.shape != ks.shape or ks.dtype != torch.float32
@@ -1102,9 +1111,6 @@ def attn_decode_fp8(q, kq, vq, ks, vs, workspace, *, length: int, length_dev=Non
     return o
 
 
-# ------------------------------------------------------------------------------------------------
-# Paged decode KV cache (serving.BatchedGenerator; the format lives in paged_kv.py)
-# ------------------------------------------------------------------------------------------------
 def _paged_pages(what, kp, vp, ksc, vsc, hd=None):
     """(fp8, num_pages, page_size, nkv, hd) of one layer's pages, after checking dtypes and shapes."""
     if kp.dim() != 4 or vp.shape != kp.shape or vp.dtype != kp.dtype or not (kp.is_contiguous() and vp.is_contiguous()):
@@ -1140,12 +1146,8 @@ def paged_kv_append(k, v, k_pages, v_pages, k_scales, v_scales, block_table, len
     """Write the new rows k, v [rows, S, nkv, hd] (views of the packed post-RoPE qkv rows, read in place) into one
     layer's pages at positions offset (+ lens[b] with offset_from_lens) + s through block_table; a row with lens[b] < 0
     writes nothing."""
-    _require_cuda_bf16(k, v)
+    ld = _kv_new_rows("paged_kv_append", k, v, "rows")
     B, S, nkv, hd = k.shape
-    ld = k.stride(1) if S > 1 else (k.stride(0) if B > 1 else nkv * hd)
-    if (v.shape != k.shape or v.stride() != k.stride() or k.stride(3) != 1 or (nkv > 1 and k.stride(2) != hd)
-            or (B > 1 and k.stride(0) != S * ld)):
-        raise ValueError(f"paged_kv_append: k, v must be [rows, S, nkv, hd] rows at one common stride, got {k.stride()}")
     fp8, num_pages, page_size, pnkv, _ = _paged_pages("paged_kv_append", k_pages, v_pages, k_scales, v_scales, hd)
     if pnkv != nkv:
         raise ValueError(f"paged_kv_append: pages hold {pnkv} kv heads, the rows {nkv}")

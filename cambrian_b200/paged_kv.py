@@ -1,7 +1,8 @@
 """Paged decode KV cache (`serving.BatchedGenerator`).
 
-This module is the one place on the host that states the format (the kernels `paged_append_kernel` and
-`paged_decode_kernel` in csrc/paged.cu are the other side).
+This module is the one place on the host that states the format (the kernels `kv_append_kernel` and `kv_decode_kernel`
+over `PagedCells` in csrc/kv_cache.cu are the other side; the dense FP8 cache of kv_fp8.py runs the same kernels over
+`DenseCells`).
 
 Pages.  Each decoder layer has a pool of `num_pages` fixed-size pages for K and one for V, each
 [num_pages, page_size, nkv, hd].  Inside a page the layout is position-major, the row layout of the dense `KVCache`: page
@@ -36,7 +37,7 @@ import torch
 
 from .kv_fp8 import CACHE_DTYPES
 
-SPLIT_KEYS = 256          # key positions per split of the decode kernel (PD_CHUNK in csrc/paged.cu)
+SPLIT_KEYS = 256          # key positions per split of the decode kernel (KVD_PAGED_CHUNK in csrc/kv_cache.cu)
 DEFAULT_PAGE_SIZE = 64
 
 

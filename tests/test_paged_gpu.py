@@ -1,7 +1,8 @@
 """GPU checks of the paged KV cache and continuous batching: the append kernel bit for bit (bf16 copy; FP8 against
 cb_kv_fp8_append) through shuffled block tables, decode attention against the fp64 reference of tests/paged_reference.py
-at hd 64 / 128, G 1 / 4 / 7 / 8 and ragged lengths up to 16k, its run-to-run determinism and batch invariance, and the
-server end to end on the peaked tiny model against solo generate()."""
+at hd 64 / 128, G 1 / 4 / 7 / 8 and ragged lengths up to 16k, its run-to-run determinism and batch invariance, its
+bitwise agreement with the dense FP8 cache's decode (cb_attn_decode_fp8), and the server end to end on the peaked tiny
+model against solo generate()."""
 import os
 import sys
 
@@ -164,6 +165,36 @@ def test_decode_is_batch_invariant(fp8):
         alone = ops.attn_decode_paged(q[b:b + 1].contiguous(), kp, vp, ks, vs, t1, lens[b:b + 1].contiguous(), ws1,
                                       len_add=1)
         assert torch.equal(alone, batch[b:b + 1]), f"row {b} alone != in the batch"
+
+
+@pytest.mark.parametrize("hd", [64, 128])
+@pytest.mark.parametrize("S_max", [1024, 2048])
+def test_decode_matches_dense_fp8_bitwise(hd, S_max):
+    """The dense FP8 cache and FP8 pages behind an identity block table share one decode arithmetic: where the dense
+    decode also splits the keys into 256-key chunks, the two outputs are equal bit for bit, for valid lengths that end
+    inside a split and at its edge."""
+    from cambrian_b200 import ops
+    B, nkv, G, ps = 1, 8, 4, 64
+    nh = nkv * G
+    ws_dense = ops.attn_decode_fp8_workspace(B, nh, nkv, S_max, hd, dev)
+    assert ws_dense.numel() == B * nh * (S_max // 256) * (hd + 2), "the dense decode does not split into 256-key chunks"
+    g = torch.Generator().manual_seed(S_max + hd)
+    x = torch.randn(2, B, S_max, nkv, hd, generator=g).to(bf)
+    x[1] *= 2.5
+    kq, ks = (t.to(dev) for t in KR.quantize_rows(x[0].float()))
+    vq, vs = (t.to(dev) for t in KR.quantize_rows(x[1].float()))
+    num_pages = S_max // ps                                          # page p holds positions [p * ps, (p + 1) * ps)
+    kp, vp = kq.view(num_pages, ps, nkv, hd), vq.view(num_pages, ps, nkv, hd)
+    kps, vps = ks.view(num_pages, ps, nkv), vs.view(num_pages, ps, nkv)
+    table = torch.arange(num_pages, dtype=torch.int32, device=dev)[None]
+    ws_paged = ops.attn_decode_paged_workspace(B, nh, num_pages, ps, hd, dev)
+    q = (torch.randn(B, 1, nh, hd, generator=g) * 1.5).to(bf).to(dev)
+    for L in (1, 255, 256, 257, 700, 768, S_max - 1, S_max):
+        dense = ops.attn_decode_fp8(q, kq, vq, ks, vs, ws_dense, length=L)
+        lens = torch.tensor([L], dtype=torch.int32, device=dev)
+        paged = ops.attn_decode_paged(q, kp, vp, kps, vps, table, lens, ws_paged, len_add=0)
+        assert dense.abs().sum() > 0
+        assert torch.equal(dense.view(torch.int16), paged.view(torch.int16)), f"hd={hd} S_max={S_max} L={L}"
 
 
 # ------------------------------------------------------------------------------------------------ end to end
