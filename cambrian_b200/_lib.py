@@ -101,6 +101,7 @@ SIGNATURES = {
     "cb_paged_kv_append": (_i, [_vp, _vp, _i64] + [_vp] * 4 + [_i, _vp, _i64, _vp] + [_i] * 7 + [_i64, _i, _vp]),
     "cb_attn_decode_paged_workspace_floats": (_i64, [_i] * 5),
     "cb_attn_decode_paged": (_i, [_vp, _i64] + [_vp] * 4 + [_i, _vp, _i64, _vp, _i, _vp, _vp, _i64] + [_i] * 7 + [_f, _vp]),
+    "cb_paged_kv_gather": (_i, [_vp] * 4 + [_i, _vp] + [_i] * 5 + [_i64, _vp, _vp, _i64, _vp]),
 }
 
 _lib = None

@@ -146,6 +146,8 @@ long long attn_decode_paged_workspace_floats(int, int, int, int, int);
 int attn_decode_paged_launch(const void*, long long, const void*, const void*, const float*, const float*, int, const int*,
                              long long, const int*, int, void*, float*, long long, int, int, int, int, int, int, int, float,
                              cudaStream_t);
+int paged_kv_gather_launch(const void*, const void*, const float*, const float*, int, const int*, int, int, int, int, int,
+                           long long, void*, void*, long long, cudaStream_t);
 
 }  // namespace cb
 
@@ -505,6 +507,12 @@ int cb_attn_decode_paged(const void* q, int64_t q_bs, const void* k_pages, const
   return cb::attn_decode_paged_launch(q, q_bs, k_pages, v_pages, k_scales, v_scales, fp8, block_table, table_ld, lens,
                                       len_add, o, workspace, workspace_floats, rows, nh, nkv, hd, page_size, num_pages,
                                       max_pages, scale, ST(stream));
+}
+int cb_paged_kv_gather(const void* k_pages, const void* v_pages, const float* k_scales, const float* v_scales, int fp8,
+                       const int* block_table_row, int nkv, int hd, int page_size, int num_pages, int max_pages, int64_t P,
+                       void* out_k, void* out_v, int64_t out_ld, void* stream) {
+  return cb::paged_kv_gather_launch(k_pages, v_pages, k_scales, v_scales, fp8, block_table_row, nkv, hd, page_size,
+                                    num_pages, max_pages, P, out_k, out_v, out_ld, ST(stream));
 }
 
 }  // extern "C"

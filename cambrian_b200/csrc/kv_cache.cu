@@ -15,6 +15,8 @@
 //                       the row rule)
 //   kv_decode_kernel    cb_attn_decode_fp8, cb_attn_decode_paged: flash-decoding, one query per row, keys split over CTAs
 //   kv_decode_combine   merges a row's splits in split order (no atomics) and rounds once to bf16
+//   kv_gather_kernel    cb_paged_kv_gather: a row's cached prefix out of the pages into dense bf16 rows (a prefix-cache
+//                       hit of the server attends over them with the flash kernel)
 #include "common.cuh"
 #include <cuda_fp16.h>
 #include <algorithm>
@@ -161,6 +163,40 @@ kv_append_kernel(const bf16* __restrict__ k, const bf16* __restrict__ v, long lo
   } else {
     *reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(which ? vc : kc) + dst) = raw;
   }
+}
+
+// Lane group r reads row r = (t * nkv + h) * 2 + (0: K, 1: V) of positions [0, P) of row 0 of the cells and writes it
+// as bf16 to out + t * ld + h * HD (16-byte stores of 8 elements per lane).  bf16 cells are copied; FP8 cells become
+// __float2bfloat16_rn(__fmul_rn(float(e4m3), scale)), one rounding per element.  A position without a cell gets zeros.
+template <int HD, bool F8, class Cells>
+__global__ void __launch_bounds__(256)
+kv_gather_kernel(const void* __restrict__ kc, const void* __restrict__ vc, const float* __restrict__ ksc,
+                 const float* __restrict__ vsc, Cells cells, int P, int nkv, bf16* __restrict__ ok, bf16* __restrict__ ov,
+                 long long ld) {
+  constexpr int LPK = HD / KV_DPL;
+  const long long r = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / LPK;
+  const int sub = threadIdx.x % LPK;
+  if (r >= 2LL * P * nkv) return;
+  const int which = (int)(r & 1);
+  const int h = (int)((r >> 1) % nkv);
+  const int t = (int)((r >> 1) / nkv);
+  const long long cell = cells.cell(0, t);
+  uint4 out = make_uint4(0u, 0u, 0u, 0u);
+  if (cell >= 0) {
+    const long long off = (cell * nkv + h) * HD + sub * KV_DPL;
+    if (F8) {
+      const uint2 q = *reinterpret_cast<const uint2*>(reinterpret_cast<const uint8_t*>(which ? vc : kc) + off);
+      const float s = (which ? vsc : ksc)[cell * nkv + h];
+      float f[8];
+      e4m3x8_to_f32(q, f);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) f[e] = __fmul_rn(f[e], s);
+      out = pack8(f);
+    } else {
+      out = *reinterpret_cast<const uint4*>(reinterpret_cast<const bf16*>(which ? vc : kc) + off);
+    }
+  }
+  *reinterpret_cast<uint4*>((which ? ov : ok) + (long long)t * ld + h * HD + sub * KV_DPL) = out;
 }
 
 // CTA (split, kv head h, row b), KVD_THREADS threads = TEAMS teams of LPK lanes.  The CTA owns the G query heads of
@@ -508,6 +544,32 @@ int attn_decode_paged_launch(const void* q, long long q_bs, const void* kp, cons
                            st);
   return kv_decode<false>(cells, hd, q, q_bs, kp, vp, ksc, vsc, o, ws, rows, nh, nkv, KVD_PAGED_CHUNK, (int)nsplit, scale,
                           st);
+}
+
+int paged_kv_gather_launch(const void* kp, const void* vp, const float* ksc, const float* vsc, int fp8, const int* table,
+                           int nkv, int hd, int page_size, int num_pages, int max_pages, long long P, void* ok, void* ov,
+                           long long out_ld, cudaStream_t st) {
+  int rc = paged_geometry("paged_kv_gather", 1, nkv, hd, page_size, num_pages, max_pages, max_pages);
+  if (rc != CB_OK) return rc;
+  const long long max_pos = (long long)max_pages * page_size;
+  CB_CHECK_ARG(P >= 0 && P <= max_pos, "paged_kv_gather: positions [0, %lld) outside the table (%lld)", P, max_pos);
+  CB_CHECK_ARG(kp && vp && table && ok && ov && (!fp8 || (ksc && vsc)), "paged_kv_gather: null argument");
+  CB_CHECK_ARG(((reinterpret_cast<uintptr_t>(kp) | reinterpret_cast<uintptr_t>(vp)) & 15u) == 0 &&
+                   ((reinterpret_cast<uintptr_t>(ok) | reinterpret_cast<uintptr_t>(ov)) & 15u) == 0 &&
+                   ((reinterpret_cast<uintptr_t>(ksc) | reinterpret_cast<uintptr_t>(vsc)) & 3u) == 0,
+               "paged_kv_gather: the pages and the outputs must be 16-byte aligned");
+  CB_CHECK_ARG(out_ld >= (long long)nkv * hd && out_ld % 8 == 0,
+               "paged_kv_gather: output row stride %lld must be >= nkv*hd and a multiple of 8", out_ld);
+  if (P == 0) return CB_OK;
+  const PagedCells cells{max_pos, 0, nullptr, 0, table, max_pages, __builtin_ctz(page_size), num_pages};
+  const long long blocks = (2LL * P * nkv * (hd / KV_DPL) + 255) / 256;
+  CB_CHECK_ARG(blocks < (1LL << 31), "paged_kv_gather: too many rows");
+  decltype(&kv_gather_kernel<64, false, PagedCells>) kern =
+      fp8 ? (hd == 128 ? kv_gather_kernel<128, true, PagedCells> : kv_gather_kernel<64, true, PagedCells>)
+          : (hd == 128 ? kv_gather_kernel<128, false, PagedCells> : kv_gather_kernel<64, false, PagedCells>);
+  kern<<<(unsigned)blocks, 256, 0, st>>>(kp, vp, ksc, vsc, cells, (int)P, nkv, (bf16*)ok, (bf16*)ov, out_ld);
+  CB_CUDA_LAUNCH_CHECK("kv_gather_kernel");
+  return CB_OK;
 }
 
 }  // namespace cb

@@ -276,11 +276,21 @@ class CBLlamaDecoderLayer(nn.Module):
 
     def _attn_paged_cache(self, q, k_new, v_new, cache, kmask):
         """Attention with the paged cache (paged_kv.py): a prefill attends over its own bf16 K / V and is then appended
-        into its empty pages; a decode step appends each row's token at lens[b], then attends over its pages."""
+        into its empty pages; a decode step appends each row's token at lens[b], then attends over its pages.  A prefill
+        after a cached prefix of P positions (a prefix-cache hit of the server) gathers [0, P) out of the pages into bf16
+        rows, puts its own bf16 K / V after them, attends over both (causal, aligned bottom-right) and appends at P."""
         kp, vp, ksc, vsc = cache.pool.layer(self.layer_idx)
         if cache.prefill:
-            attn = ops.attn_fwd(q, k_new, v_new, causal=True, kmask=kmask)
-            ops.paged_kv_append(k_new, v_new, kp, vp, ksc, vsc, cache.table, offset=0)
+            P = cache.prefix
+            if P:
+                kb, vb = cache.prefix_buffers(k_new.shape[1], self.nkv, self.hd, q.device)
+                ops.paged_kv_gather(kp, vp, ksc, vsc, cache.table[0], P, kb, vb)
+                kb[:, P:].copy_(k_new)
+                vb[:, P:].copy_(v_new)
+                attn = ops.attn_fwd(q, kb, vb, causal=True, kmask=kmask)
+            else:
+                attn = ops.attn_fwd(q, k_new, v_new, causal=True, kmask=kmask)
+            ops.paged_kv_append(k_new, v_new, kp, vp, ksc, vsc, cache.table, offset=P)
             return attn
         ops.paged_kv_append(k_new, v_new, kp, vp, ksc, vsc, cache.table, cache.lens, offset_from_lens=True)
         return ops.attn_decode_paged(q, kp, vp, ksc, vsc, cache.table, cache.lens, cache.pool.ws, len_add=1)
@@ -646,12 +656,19 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
         self.train(was_training)
         return torch.stack(tokens, 1)
 
-    def _prefill(self, inputs, images, image_sizes, attention_mask, position_ids, kwargs, make_cache):
+    def _prefill(self, inputs, images, image_sizes, attention_mask, position_ids, kwargs, make_cache, prefix: int = 0):
         """The prefill of generate() and of serving.BatchedGenerator: multimodal preparation (towers, connector, splice),
         the generation keywords (GenerationArgs, which needs the spliced prompt length S0), the cache from
         make_cache(B, S0, max_new_tokens), the prefill forward over it, and each row's last hidden state and next
-        position.  Returns (args, cache, h_last [B, H], next_pos [B], S0)."""
+        position.  Returns (args, cache, h_last [B, H], next_pos [B], S0).
+
+        prefix > 0 (the server's prefix-cache hit): the cache already holds positions [0, prefix) of the one sequence and
+        `inputs` are the text ids of positions prefix .. S0-1 (S0 = prefix + n), so no image preparation runs; the
+        keywords and the cache mask see the whole S0."""
         from ...generation import GenerationArgs
+        if prefix and (images is not None or attention_mask is not None or position_ids is not None
+                       or inputs.shape[0] != 1):
+            raise ValueError("a prefill after a cached prefix takes one unpadded text-only sequence")
         feats = masks = final_size = ctx_feat = None
         if images is not None:
             (_, position_ids, attention_mask, _, inputs_embeds, _, feats, masks, final_size, ctx_feat) = \
@@ -660,7 +677,8 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
         else:
             inputs_embeds = None
         B = inputs.shape[0]
-        S0 = inputs_embeds.shape[1] if inputs_embeds is not None else inputs.shape[1]
+        n = inputs_embeds.shape[1] if inputs_embeds is not None else inputs.shape[1]
+        S0 = prefix + n
         args = GenerationArgs.from_kwargs(self, S0, kwargs)
         max_new = args.max_new_tokens
         dev = inputs.device
@@ -675,7 +693,7 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
                          vision_tower_aux_feature_list=feats, vision_tower_aux_attention_masks_list=masks,
                          final_vision_feature_size=final_size, global_context_feature=ctx_feat)
         last_idx = (cache.kmask[:, :S0].long().cumsum(1).argmax(1)) if attention_mask is not None else \
-            torch.full((B,), S0 - 1, device=dev)
+            torch.full((B,), n - 1, device=dev)
         h_last = out.last_hidden_state[torch.arange(B, device=dev), last_idx].contiguous()
         next_pos = (position_ids.max(1).values + 1) if position_ids is not None else torch.full((B,), S0, device=dev)
         return args, cache, h_last, next_pos, S0

@@ -1185,3 +1185,22 @@ def attn_decode_paged(q, k_pages, v_pages, k_scales, v_scales, block_table, lens
                                            workspace.numel(), B, nh, nkv, hd, page_size, num_pages, max_pages,
                                            float(scale), stream()), "cb_attn_decode_paged")
     return o
+
+
+def paged_kv_gather(k_pages, v_pages, k_scales, v_scales, block_table_row, P: int, out_k, out_v):
+    """Positions [0, P) of one block-table row (int32 [max_pages]) out of one layer's pages into out_k, out_v
+    [>= P, nkv, hd] bf16 (row stride >= nkv * hd, e.g. the head of a [1, P + n, nkv, hd] buffer): bf16 pages are copied,
+    FP8 pages dequantised to bf16(float(e4m3) * scale), one rounding per element."""
+    fp8, num_pages, page_size, nkv, hd = _paged_pages("paged_kv_gather", k_pages, v_pages, k_scales, v_scales)
+    if block_table_row.dim() != 1 or block_table_row.dtype != torch.int32 or not block_table_row.is_contiguous():
+        raise ValueError("paged_kv_gather: block_table_row must be a contiguous int32 [max_pages]")
+    _require_cuda_bf16(out_k, out_v)
+    if out_k.dim() == 4 and out_k.shape[0] == 1 and out_v.dim() == 4:      # [1, P + n, nkv, hd] buffers
+        out_k, out_v = out_k[0], out_v[0]
+    if (out_k.dim() != 3 or out_k.shape[1:] != (nkv, hd) or out_v.shape != out_k.shape or out_v.stride() != out_k.stride()
+            or out_k.shape[0] < P or out_k.stride(2) != 1 or out_k.stride(1) != hd):
+        raise ValueError(f"paged_kv_gather: out_k, out_v must be [>= {P}, {nkv}, {hd}] bf16 at one common row stride")
+    ld = out_k.stride(0) if out_k.shape[0] > 1 else nkv * hd
+    check(_lib.load().cb_paged_kv_gather(ptr(k_pages), ptr(v_pages), ptr(k_scales), ptr(v_scales), fp8,
+                                         ptr(block_table_row), nkv, hd, page_size, num_pages, block_table_row.shape[0],
+                                         int(P), ptr(out_k), ptr(out_v), ld, stream()), "cb_paged_kv_gather")

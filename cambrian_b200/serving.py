@@ -30,9 +30,32 @@ bitwise independent of the other rows.  The rest of the step is not: the project
 by the bucket's row count (ops.gemm: the CUDA-core GEMV up to 8 rows, except wide outputs at 6-8 rows; the tensor-core
 GEMM above), and those kernels sum in different orders.  So a request's logits can change in the last bits with the
 number of requests running beside it, and a close greedy race can then go the other way.
+
+Prefix cache (`prefix_cache=True`, off by default; paged_kv.py states the index).  Multi-turn chat resends the whole
+conversation with its image, and several questions about one image repeat the system prompt and the image; a hit
+reuses those cached pages instead of running the towers, the connector, the SVA sites and the prefill over them.
+  * Contents.  A request's prompt contents are its ids with the <image> indicator expanded to the image's span, every
+    span position carrying the image digest: SHA-256 of the host bytes, dtypes and shapes of the per-tower image
+    tensors plus `image_sizes`, computed at `submit`.  The span length is learned from the first prefill of the
+    image (the dynamic branch makes it depend on `image_sizes`, which the digest includes).
+  * Matching, when the request reaches the head of the queue: whole matching pages of the index, then the longest
+    match of leading rows inside one more indexed page, whose rows are copied into the request's first private page.
+    The hit is capped at S0 - 1 positions, so at least one position is prefilled and gives the first token.
+  * Image rule.  A request with an image hits only if the hit covers its whole image span, since the in-LLM SVA sites
+    address the span at `cfg.image_position` of the forward's own hidden states; otherwise it gets a full prefill.  An
+    image request whose span length is not known yet, whose ids already hold an expanded span, or whose <image> is not
+    at `image_position` while SVA sites run, is served without the cache.  Text-only requests hit on any prefix.
+  * Admission references the matched pages before it allocates, so it never evicts its own hit, and reserves
+    pages_for(S0 + max_new_tokens) minus the shared whole pages (S0 is exact on a hit).  Retirement drops the
+    references: indexed pages become cached-idle, the others free.
+  * Numerics.  A miss is bitwise the server without the cache.  A hit's first-token logits are not bitwise a miss's:
+    the suffix's projections see n rows (ops.gemm takes the GEMV at 8 rows or fewer), the flash kernel runs with
+    Sq < Skv over the gathered prefix, and FP8 prefix rows are dequantised once to bf16.
+  * `hit_rate()` is reused prompt positions over prefilled prompt positions; `cached_pages()` the index's size.
 """
 from __future__ import annotations
 
+import hashlib
 from collections import deque
 from dataclasses import dataclass, field
 
@@ -41,7 +64,8 @@ import torch
 from . import ops
 from .generation import GenerationArgs, next_tokens, should_stop
 from .kv_fp8 import resolve_cache_dtype
-from .paged_kv import DEFAULT_PAGE_SIZE, PagedCacheView, PagedKVPool, check_page_size, pages_for
+from .model.cambrian_arch import IMAGE_TOKEN_INDEX
+from .paged_kv import DEFAULT_PAGE_SIZE, ROOT, PagedCacheView, PagedKVPool, check_page_size, pages_for
 
 
 @dataclass
@@ -58,13 +82,22 @@ class _Request:
     tokens: list = field(default_factory=list)
     length: int = 0                 # cached positions
     pos: int = 0                    # position id of the next decode token
+    # prefix cache (prefix_cache=True)
+    host_ids: list = None           # the prompt ids on the host
+    digest: bytes = None            # the image digest (None: no image, or an image the cache cannot key)
+    content: list = None            # the prompt's position contents after the splice (None: not known)
+    image_end: int = 0              # the first position after the image span (0: no image)
+    prefix: int = 0                 # positions reused from the index at admission
+    node: int = ROOT                # the index node of the request's leading indexed pages
+    indexed: int = 0                # leading pages of the request that are in the index
+    held: list = field(default_factory=list)   # index pages referenced in place of its own pages of equal contents
 
 
 class BatchedGenerator:
     """Serve generation requests of one model at once over a paged KV cache (see the module docstring)."""
 
     def __init__(self, model, max_batch: int = 32, max_cached_tokens: int = 65536, page_size: int = DEFAULT_PAGE_SIZE,
-                 kv_cache_dtype: str | None = None, use_graph: bool = True):
+                 kv_cache_dtype: str | None = None, use_graph: bool = True, prefix_cache: bool = False):
         from .model.language_model.cambrian_phi3 import CambrianPhi3ForCausalLM
         if isinstance(model, CambrianPhi3ForCausalLM):
             raise NotImplementedError("BatchedGenerator does not serve Cambrian-Phi3 yet: the paged decode kernel has no "
@@ -102,6 +135,9 @@ class BatchedGenerator:
         self._dirty = True           # the row set changed since lens / pos / table were last uploaded
         q_num = int(getattr(cfg, "image_token_len", 576))
         self._image_extra = q_num + int(q_num ** 0.5) - 1
+        self.prefix_cache = bool(prefix_cache)
+        self.prompt_positions = 0    # prompt positions of the prefilled requests
+        self.reused_positions = 0    # of those, positions taken from the prefix index instead of being prefilled
 
     # ------------------------------------------------------------------------------------------------ public API
     def nbytes(self) -> int:
@@ -110,6 +146,14 @@ class BatchedGenerator:
 
     def free_pages(self) -> int:
         return self.pool.free_pages()
+
+    def cached_pages(self) -> int:
+        """Pages in the prefix index (referenced or cached-idle)."""
+        return self.pool.cached_pages()
+
+    def hit_rate(self) -> float:
+        """Prompt positions reused from the prefix index over all prompt positions prefilled so far."""
+        return self.reused_positions / max(self.prompt_positions, 1)
 
     def pending(self) -> int:
         """Requests submitted and not finished (queued or running)."""
@@ -140,7 +184,12 @@ class BatchedGenerator:
                              f"{self.pool.max_pages_per_seq} per sequence, positions up to {self.max_pos}")
         rid = self._next_rid
         self._next_rid += 1
-        self._queue.append(_Request(rid, ids.to(self.device), images, image_sizes, dict(kwargs), args, need))
+        r = _Request(rid, ids.to(self.device), images, image_sizes, dict(kwargs), args, need)
+        if self.prefix_cache:
+            r.host_ids = ids[0].tolist()
+            if images is not None:
+                r.digest = _image_digest(images, image_sizes)
+        self._queue.append(r)
         return rid
 
     @torch.no_grad()
@@ -171,10 +220,27 @@ class BatchedGenerator:
     # ------------------------------------------------------------------------------------------------ internals
     def _admit(self):
         events = []
-        while (self._queue and len(self._active) < self.max_batch
-               and self.pool.free_pages() >= self._queue[0].reserve):
-            r = self._queue.popleft()
-            r.pages = self.pool.alloc(r.reserve)
+        while self._queue and len(self._active) < self.max_batch:
+            r = self._queue[0]
+            hit = self._match(r) if self.prefix_cache else None
+            if hit is None:
+                if self.pool.free_pages() < r.reserve:
+                    break
+                self._queue.popleft()
+                r.pages = self.pool.alloc(r.reserve)
+            else:
+                shared, src, P, reserve = hit
+                held = shared + ([src] if src is not None else [])
+                # the matched pages are referenced before the allocation, so it cannot evict them
+                if self.pool.free_pages() - self.pool.idle_among(held) < reserve:
+                    break
+                self._queue.popleft()
+                self.pool.ref(held)
+                r.pages = shared + self.pool.alloc(reserve)
+                if src is not None:
+                    self._copy_rows(src, r.pages[len(shared)], P % self.page_size)
+                    self.pool.release([src])
+                r.prefix, r.node, r.indexed = P, (shared[-1] if shared else ROOT), len(shared)
             try:
                 events.append(self._prefill(r))
             except BaseException:
@@ -185,12 +251,90 @@ class BatchedGenerator:
                 raise
         return events
 
+    # ---- prefix cache ----
+    def _content(self, r: _Request):
+        """The request's prompt position contents after the splice (token ids; the image digest over its span), or
+        None while its image's span length is unknown or when the cache cannot key the request."""
+        if r.content is not None or r.host_ids is None:
+            return r.content
+        ids = r.host_ids
+        if r.images is None:
+            r.content = list(ids)
+            return r.content
+        span = self.pool.image_span.get(r.digest) if r.digest is not None else None
+        if span is None or ids.count(IMAGE_TOKEN_INDEX) != 1:
+            return None
+        p0 = ids.index(IMAGE_TOKEN_INDEX)
+        cfg = self.model.config
+        if not getattr(cfg, "connector_only", True) and p0 != getattr(cfg, "image_position", p0):
+            return None         # the in-LLM SVA sites would rewrite positions outside the image span
+        if (getattr(cfg, "inputs_pre_expanded", False)
+                or (p0 + span <= len(ids) and not any(ids[p0 + 1:p0 + span]))):
+            return None         # an already expanded span: the splice keeps the ids' length
+        content = ids[:p0] + [r.digest] * span + ids[p0 + 1:]
+        max_tok = getattr(cfg, "tokenizer_model_max_length", None)
+        if max_tok is not None and len(content) > max_tok:
+            return None         # the splice truncates
+        r.content, r.image_end = content, p0 + span
+        return content
+
+    def _match(self, r: _Request):
+        """(shared pages, partial source page or None, P, private pages to reserve) of the request's hit, or None."""
+        C = self._content(r)
+        if C is None:
+            return None
+        ps, S0 = self.page_size, len(C)
+        full, part = self.pool.match(C)
+        P = min(len(full) * ps + (part[1] if part is not None else 0), S0 - 1)
+        if P <= 0 or P < r.image_end:
+            return None         # no hit, or a hit that ends before the end of the image span
+        nfull = P // ps
+        src = None
+        if P % ps:
+            src = full[nfull] if nfull < len(full) else part[0]
+        max_new = GenerationArgs.from_kwargs(self.model, S0, r.kwargs).max_new_tokens
+        return full[:nfull], src, P, pages_for(S0 + max_new, ps) - nfull
+
+    def _copy_rows(self, src: int, dst: int, rows: int):
+        """The first `rows` positions of page src into page dst, in every layer (FP8: bytes and scales)."""
+        for i in range(len(self.pool.k)):
+            for t in self.pool.layer(i):
+                if t is not None:
+                    t[dst, :rows].copy_(t[src, :rows])
+
+    def _index(self, r: _Request):
+        """Index the request's pages whose positions are all written (prompt contents, then generated tokens)."""
+        if r.content is None:
+            return
+        ps = self.page_size
+        S0 = len(r.content)
+        while (r.indexed + 1) * ps <= r.length:
+            a, b = r.indexed * ps, (r.indexed + 1) * ps
+            key = tuple(r.content[a:b] if b <= S0 else r.content[a:] + r.tokens[:b - S0])
+            page = r.pages[r.indexed]
+            r.node = self.pool.insert(r.node, key, page)
+            if r.node != page:          # indexed already (by a request that prefilled the same prompt): hold that page
+                self.pool.ref([r.node])
+                r.held.append(r.node)
+            r.indexed += 1
+
+    def _learn(self, r: _Request, S0: int):
+        """After a miss's prefill: learn its image's span length and its contents, if the cache can key it."""
+        if r.host_ids is None or r.content is not None:
+            return
+        if r.digest is not None and r.digest not in self.pool.image_span and r.host_ids.count(IMAGE_TOKEN_INDEX) == 1:
+            span = S0 - len(r.host_ids) + 1
+            if span > 1:
+                self.pool.image_span[r.digest] = span
+        if self._content(r) is not None and len(r.content) != S0:
+            r.content = None
+
     def _prefill(self, r: _Request):
         mpps = self.pool.max_pages_per_seq
         r.table = torch.zeros(mpps, dtype=torch.int32)
         r.table[:len(r.pages)] = torch.tensor(r.pages, dtype=torch.int32)
         table = r.table.view(1, mpps).to(self.device)
-        view = PagedCacheView(self.pool, table, None, prefill=True)
+        view = PagedCacheView(self.pool, table, None, prefill=True, prefix=r.prefix)
         reserved = len(r.pages) * self.page_size
 
         def make_cache(B, S0, max_new):
@@ -198,16 +342,27 @@ class BatchedGenerator:
                 raise RuntimeError(f"prefill of {S0} positions + {max_new} new tokens exceeds the {reserved} reserved")
             return view
 
-        args, _, h_last, next_pos, S0 = self.model._prefill(r.ids, r.images, r.image_sizes, None, None, r.kwargs,
-                                                            make_cache)
+        if r.prefix:
+            # a hit covers any image span: the suffix is text only and runs without the towers
+            suffix = torch.tensor([r.content[r.prefix:]], dtype=torch.long, device=self.device)
+            args, _, h_last, next_pos, S0 = self.model._prefill(suffix, None, None, None, None, r.kwargs, make_cache,
+                                                                prefix=r.prefix)
+        else:
+            args, _, h_last, next_pos, S0 = self.model._prefill(r.ids, r.images, r.image_sizes, None, None, r.kwargs,
+                                                                make_cache)
         r.args = args
         keep = pages_for(S0 + args.max_new_tokens, self.page_size)
         if keep < len(r.pages):
             self.pool.release(r.pages[keep:])
             r.table[keep:] = 0
             r.pages = r.pages[:keep]
-        r.images = r.image_sizes = None
         r.length, r.pos = S0, int(next_pos.reshape(-1)[0])
+        if self.prefix_cache:
+            self._learn(r, S0)
+            self._index(r)
+            self.prompt_positions += S0
+            self.reused_positions += r.prefix
+        r.images = r.image_sizes = None
         if args.streamer is not None:
             args.streamer.put(torch.empty((1, 0), dtype=torch.long))     # HF streams the (here: empty) prompt ids first
         logits = ops.gemm(h_last, self.model.lm_head.weight, out_dtype=torch.float32)
@@ -233,8 +388,8 @@ class BatchedGenerator:
         return done
 
     def _retire(self, r: _Request):
-        self.pool.release(r.pages)
-        r.pages = []
+        self.pool.release(r.pages + r.held)
+        r.pages, r.held = [], []
         if r.args.streamer is not None:
             r.args.streamer.end()
         self._results[r.rid] = torch.tensor(r.tokens, dtype=torch.long)
@@ -302,6 +457,8 @@ class BatchedGenerator:
         for i, (r, tok) in enumerate(zip(act, toks)):
             r.length += 1
             r.pos += 1
+            if self.prefix_cache:
+                self._index(r)      # a page whose last position this step wrote
             finished = self._emit(r, tok, logits[i:i + 1])
             if finished:
                 self._retire(r)
@@ -312,3 +469,17 @@ class BatchedGenerator:
             self._active = keep
             self._dirty = True
         return events
+
+
+def _image_digest(images, image_sizes) -> bytes | None:
+    """SHA-256 of the request's per-tower image tensors (host bytes, dtype, shape) and image_sizes; None when an image
+    is not a tensor."""
+    h = hashlib.sha256()
+    for t in ([images] if torch.is_tensor(images) else list(images)):
+        if not torch.is_tensor(t):
+            return None
+        t = t.detach().contiguous().cpu()
+        h.update(repr((str(t.dtype), tuple(t.shape))).encode())
+        h.update(t.view(torch.uint8).numpy().tobytes() if t.numel() else b"")
+    h.update(repr(None if image_sizes is None else [tuple(int(x) for x in s) for s in image_sizes]).encode())
+    return h.digest()

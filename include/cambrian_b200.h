@@ -436,6 +436,15 @@ int cb_attn_decode_paged(const void* q, int64_t q_bs, const void* k_pages, const
                          const float* v_scales, int fp8, const int* block_table, int64_t table_ld, const int* lens,
                          int len_add, void* o, float* workspace, int64_t workspace_floats, int rows, int nh, int nkv, int hd,
                          int page_size, int num_pages, int max_pages, float scale, void* stream);
+/* Gather positions [0, P) of one block-table row (block_table_row: max_pages int32 entries) out of one layer's pages into
+ * dense bf16 rows: position t, kv head h at out + t * out_ld + h * hd (out_ld >= nkv * hd, a multiple of 8, so the
+ * outputs can be the head of a [1, P + n, nkv, hd] buffer).  bf16 pages are copied; FP8 pages are dequantised as
+ * __float2bfloat16_rn(__fmul_rn(float(e4m3), scale)), one rounding per element.  A position whose table entry is not a
+ * page of the pool gets zeros.  P <= max_pages * page_size; P = 0 launches nothing.  The pages and outputs are 16-byte
+ * aligned.  Used by the server's prefix cache: a hit attends over the gathered prefix with the flash kernel. */
+int cb_paged_kv_gather(const void* k_pages, const void* v_pages, const float* k_scales, const float* v_scales, int fp8,
+                       const int* block_table_row, int nkv, int hd, int page_size, int num_pages, int max_pages, int64_t P,
+                       void* out_k, void* out_v, int64_t out_ld, void* stream);
 
 #ifdef __cplusplus
 }

@@ -3,6 +3,7 @@
 same seeded request mix, in one session, alternated.
 
     python tools/serve_bench.py [--requests 64] [--max-batch 32] [--rounds 2] [--load-fp8] [--kv-fp8] [--out FILE]
+                                [--prefix-cache] [--mix random|shared]
 
 The mix: every request has one image and a text prompt of 64-448 tokens (at least the config's image position, 91
 for the 8B config; plus the 600-position image span), and
@@ -15,6 +16,17 @@ so its page pool and its per-bucket CUDA graphs are built before the clock start
 `generate()` call builds its own cache and graph inside its timed run, as it does in use.  Each request's greedy tokens are compared with the
 sequential run's: where they differ, the first differing step and the sequential run's top-1 / top-2 logit margin there.
 The card's name, power limit and max SM clock are read in the same call and printed with the numbers.
+`--prefix-cache` serves the random mix with BatchedGenerator(prefix_cache=True) (its prompts share nothing, so this
+measures the cache's bookkeeping).
+
+`--mix shared` measures the prefix cache on the traffic it is for: per round, 8 images with 6 questions each (one system
+prompt up to the image position, the image, a question of 8-64 tokens) and 8 three-turn conversations about their own
+image (each turn resends the previous turn, its answer and a new question), arriving in three waves: the first turns
+with all questions, then the second turns, then the third.  Two servers, one with the prefix cache and one without,
+are each warmed up once on a mix of another seed and then timed alternately, each round on a fresh mix (so no round
+hits on pages of an earlier one).  Reported per server: generated tokens / s, mean and p90 time to first token (from a
+wave's submit to the request's first token), the hit rate and cached pages; then the gather kernel's time (CUDA events)
+at the mix's hit lengths, with its bytes / s against 3.35 TB/s.
 """
 import argparse
 import json
@@ -83,13 +95,21 @@ def timed(fn):
     return out, time.perf_counter() - t0, torch.cuda.max_memory_allocated()
 
 
-def make_server(model, args, kv):
+def make_server(model, args, kv, prefix_cache=False):
     """One server for the warm-up and every timed run: its page pool and its per-bucket CUDA graphs are built once, in
-    the warm-up.  `srv.lat` collects the host time of each decode step by bucket (reset after the warm-up)."""
+    the warm-up.  `srv.lat` collects the host time of each decode step by bucket (reset after the warm-up), `srv.hits`
+    the positions each prefill reused."""
     from cambrian_b200.serving import BatchedGenerator
     srv = BatchedGenerator(model, max_batch=args.max_batch, max_cached_tokens=args.max_cached_tokens, page_size=64,
-                           kv_cache_dtype=kv)
-    srv.lat = {}
+                           kv_cache_dtype=kv, prefix_cache=prefix_cache)
+    srv.lat, srv.hits = {}, []
+    prefill = srv._prefill
+
+    def record(r):
+        srv.hits.append(r.prefix)
+        return prefill(r)
+
+    srv._prefill = record
     inner = srv._decode
 
     def decode():
@@ -189,6 +209,124 @@ def attn_kernel(srv, reqs, args, iters=50):
                 share_of_3_35_tb_s=nbytes / us / 1e6 / 3.35)
 
 
+# ------------------------------------------------------------------------------------------------ --mix shared
+def shared_mix(cfg, seed, dev, images=8, questions=6, convs=8):
+    """[dict(ids, images, new, turn, prev)]: questions on shared images (turn 0) and conversation turns 0..2 (`prev`: the
+    index of the previous turn, whose prompt and answer the turn's prompt starts with)."""
+    g = torch.Generator().manual_seed(seed)
+    res = bench.CONFIGS["8b-ddp"]["res"]
+    system = torch.randint(3, cfg.vocab_size, (cfg.image_position,), generator=g)
+    tok = lambda lo, hi: torch.randint(3, cfg.vocab_size, (int(torch.randint(lo, hi, (1,), generator=g)),),  # noqa: E731
+                                       generator=g)
+    new = lambda: int(torch.randint(16, 129, (1,), generator=g))  # noqa: E731
+    image = lambda: [torch.randn(1, 3, r, r, generator=g).bfloat16().to(dev) for r in res]  # noqa: E731
+    out = []
+    for _ in range(images):
+        img = image()
+        for _ in range(questions):
+            out.append(dict(ids=torch.cat([system, torch.tensor([-200]), tok(8, 65)]), images=img, new=new(), turn=0,
+                            prev=None))
+    for _ in range(convs):
+        img = image()
+        out.append(dict(ids=torch.cat([system, torch.tensor([-200]), tok(8, 65)]), images=img, new=new(), turn=0,
+                        prev=None))
+        for t in (1, 2):
+            out.append(dict(ids=tok(8, 33), images=img, new=new(), turn=t, prev=len(out) - 1))
+    return out
+
+
+def run_shared(srv, mix):
+    """The mix in three waves (turn 0, 1, 2); returns (tokens per request, time to first token per request in s)."""
+    answers, prompts, ttft = {}, {}, {}
+    for turn in range(3):
+        wave = [i for i, r in enumerate(mix) if r["turn"] == turn]
+        rid = {}
+        t0 = time.perf_counter()
+        for i in wave:
+            r = mix[i]
+            p = r["ids"] if r["prev"] is None else torch.cat([prompts[r["prev"]], torch.tensor(answers[r["prev"]]),
+                                                               r["ids"]])
+            prompts[i] = p
+            rid[srv.submit(p.to(srv.device), images=r["images"], image_sizes=[(336, 336)], max_new_tokens=r["new"],
+                           do_sample=False, eos_token_id=None)] = i
+        while srv.pending():
+            for q, _, _ in srv.step():                 # step() ends in a host read of the tokens (a synchronise)
+                if rid.get(q) is not None and rid[q] not in ttft:
+                    ttft[rid[q]] = time.perf_counter() - t0
+        outs = srv.run()
+        answers.update({rid[q]: t.tolist() for q, t in outs.items()})
+    return [answers[i] for i in range(len(mix))], [ttft[i] for i in range(len(mix))]
+
+
+def gather_kernel(srv, lengths, iters=50):
+    """One layer's cb_paged_kv_gather at the given prefix lengths, CUDA events around `iters` launches replayed from one
+    CUDA graph (so the host's per-call checks do not pace the device); bytes = K + V rows (+ scales) read and the bf16
+    rows written."""
+    from cambrian_b200 import ops
+    cfg = srv.model.config
+    pool = srv.pool
+    nkv = cfg.num_key_value_heads
+    hd = cfg.hidden_size // cfg.num_attention_heads
+    row = torch.arange(pool.max_pages_per_seq, dtype=torch.int32, device=srv.device) % pool.num_pages
+    kp, vp, ks, vs = pool.layer(0)
+    out = []
+    for P in lengths:
+        ok = torch.empty((1, P, nkv, hd), dtype=torch.bfloat16, device=srv.device)
+        ov = torch.empty_like(ok)
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            ops.paged_kv_gather(kp, vp, ks, vs, row, P, ok, ov)
+        torch.cuda.current_stream().wait_stream(side)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            for _ in range(iters):
+                ops.paged_kv_gather(kp, vp, ks, vs, row, P, ok, ov)
+        graph.replay()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        graph.replay()
+        e1.record()
+        torch.cuda.synchronize()
+        us = e0.elapsed_time(e1) * 1e3 / iters
+        nbytes = 2 * P * nkv * (hd * (1 if pool.fp8 else 2) + (4 if pool.fp8 else 0) + hd * 2)
+        out.append(dict(P=P, us=us, us_all_layers=us * cfg.num_hidden_layers, bytes=nbytes, gb_s=nbytes / us / 1e3,
+                        share_of_3_35_tb_s=nbytes / us / 1e6 / 3.35))
+    return out
+
+
+def main_shared(args, dev, card, cfg, model, kv):
+    servers = {pc: make_server(model, args, kv, prefix_cache=pc) for pc in (True, False)}
+    for pc, srv in servers.items():
+        run_shared(srv, shared_mix(cfg, args.seed + 1000, dev))            # warm-up: pool, graphs, allocator
+    lines, tokens = [], {}
+    for rnd in range(args.rounds):
+        mix = shared_mix(cfg, args.seed + rnd, dev)
+        n_tokens = sum(r["new"] for r in mix)
+        for pc, srv in servers.items():
+            srv.hits = []
+            reused, prompt = srv.reused_positions, srv.prompt_positions
+            (toks, ttft), wall, peak = timed(lambda: run_shared(srv, mix))
+            tokens[pc] = toks
+            ttft = sorted(ttft)
+            line = dict(way="server", mix="shared", prefix_cache=pc, round=rnd, requests=len(mix),
+                        generated_tokens=n_tokens, wall_s=wall, tokens_per_s=n_tokens / wall,
+                        ttft_mean_ms=1e3 * sum(ttft) / len(ttft), ttft_p90_ms=1e3 * ttft[int(0.9 * (len(ttft) - 1))],
+                        hit_rate=(srv.reused_positions - reused) / max(srv.prompt_positions - prompt, 1),
+                        cached_pages=srv.cached_pages(), page_pool_bytes=srv.nbytes(), peak_alloc_bytes=peak,
+                        kv_cache_dtype=kv, load_fp8=args.load_fp8, max_batch=args.max_batch, card=card)
+            lines.append(line)
+            print(json.dumps(line), flush=True)
+    hits = sorted(h for h in servers[True].hits if h > 0)
+    lengths = sorted({hits[0], hits[len(hits) // 2], hits[-1]}) if hits else []
+    same = sum(a == b for a, b in zip(tokens[True], tokens[False]))
+    summary = dict(metric="serve_shared_summary", card=card, gather_kernel=gather_kernel(servers[True], lengths),
+                   hits=len(hits), requests=len(tokens[True]), equal_tokens_with_and_without_cache=same)
+    lines.append(summary)
+    print(json.dumps(summary), flush=True)
+    return lines
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--requests", type=int, default=64)
@@ -199,6 +337,9 @@ def main():
     ap.add_argument("--load-fp8", action="store_true", help="FP8 E4M3 decoder projections (quant_fp8)")
     ap.add_argument("--kv-fp8", action="store_true", help="FP8 pages / FP8 KV cache instead of bf16")
     ap.add_argument("--out", default=None, help="also write the JSON lines to this file")
+    ap.add_argument("--prefix-cache", action="store_true", help="serve the random mix with prefix_cache=True")
+    ap.add_argument("--mix", choices=("random", "shared"), default="random",
+                    help="shared: the prefix cache's workload, with and without the cache (module docstring)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("serve_bench.py measures on a GPU; none is visible")
@@ -207,11 +348,18 @@ def main():
     card = card_info()
     cfg, model = build_model(args, dev)
     kv = "fp8" if args.kv_fp8 else "bf16"
+    if args.mix == "shared":
+        lines = main_shared(args, dev, card, cfg, model, kv)
+        if args.out:
+            with open(args.out, "w") as f:
+                for ln in lines:
+                    f.write(json.dumps(ln) + "\n")
+        return
     reqs = request_mix(cfg, args.requests, args.seed, dev)
     n_tokens = sum(r["new"] for r in reqs)
     # warm-up of every path (kernel attributes, allocator); the server's warm-up fills every bucket from max_batch down to
     # 1 as its requests retire, so the timed runs replay graphs captured here and allocate no pages
-    srv = make_server(model, args, kv)
+    srv = make_server(model, args, kv, prefix_cache=args.prefix_cache)
     warm = reqs[:min(len(reqs), args.max_batch)]
     run_server(srv, warm)
     captured = sorted(srv._graphs)
@@ -233,6 +381,7 @@ def main():
                         tokens_per_s=n_tokens / wall, peak_alloc_bytes=peak, kv_cache_dtype=kv, load_fp8=args.load_fp8,
                         max_batch=args.max_batch, card=card)
             if way == "server":
+                line["prefix_cache"] = args.prefix_cache
                 line["page_pool_bytes"] = srv.nbytes()
                 line["graphs_captured_in_timed_run"] = len(srv._graphs) - n_graphs
             lines.append(line)
