@@ -488,6 +488,8 @@ def tower_combine_fwd(logits, aggs, q_in):
     logits [N, >= T] bf16 (extra columns are padding), aggs: T tensors [N, C], q_in [N, C]."""
     _require_cuda_bf16(logits, q_in, *aggs)
     N, C_ = q_in.shape
+    if not q_in.is_contiguous():
+        raise ValueError("tower_combine_fwd: q_in must be contiguous (the kernel reads it at row stride C)")
     if logits.shape[0] != N or logits.stride(1) != 1 or any(a.shape != q_in.shape or not a.is_contiguous() for a in aggs):
         raise ValueError("tower_combine_fwd: logits [N, Tpad] and T contiguous aggregates shaped like q_in are required")
     out = torch.empty_like(q_in)
@@ -502,6 +504,10 @@ def tower_combine_bwd(logits, aggs, dout):
     N, C_ = dout.shape
     if not logits.is_contiguous() or not dout.is_contiguous():
         raise ValueError("tower_combine_bwd: contiguous logits / dout are required")
+    if logits.dim() != 2 or logits.shape[0] != N or logits.shape[1] > 32:
+        raise ValueError(f"tower_combine_bwd: logits {tuple(logits.shape)} must be [N={N}, Tpad <= 32]")
+    if any(a.shape != dout.shape or not a.is_contiguous() for a in aggs):
+        raise ValueError("tower_combine_bwd: T contiguous aggregates shaped like dout are required")
     daggs = [torch.empty_like(a) for a in aggs]
     dlogits = torch.empty_like(logits)
     check(_lib.load().cb_tower_combine_bwd(ptr(logits), logits.stride(0), ptr_array(aggs), ptr(dout), ptr_array(daggs),

@@ -282,8 +282,9 @@ int cb_clip_coef(float* sumsq, float max_norm, float inv_world, float* coef, voi
  * of the weight_mlp logits and the weighted sum of the per-tower aggregates added to the query stream,
  *   out[n,:] = q_in[n,:] + sum_t softmax(logits[n,:T])[t] * aggs[t][n,:]        (replaces .softmax(-1), torch.stack,
  * (agg * weight).sum(2) and the residual add).  logits [N, ld_logits >= T] bf16 (columns >= T are padding), aggs = HOST
- * array of T device pointers to [N, C] bf16.  Backward: daggs[t] = w_t * dout, dlogits = softmax adjoint of
- * g_t = <dout, agg_t> (padding columns zeroed); d q_in = dout. */
+ * array of T device pointers to [N, C] bf16; q_in, out, dout and daggs[t] are [N, C] bf16 at row stride C.  Backward:
+ * daggs[t] = w_t * dout, dlogits [N, ld_logits <= 32] = softmax adjoint of g_t = <dout, agg_t> (padding columns zeroed);
+ * d q_in = dout. */
 int cb_tower_combine_fwd(const void* logits, int ld_logits, const void* const* aggs, const void* q_in, void* out, int64_t N,
                          int C, int num_towers, void* stream);
 int cb_tower_combine_bwd(const void* logits, int ld_logits, const void* const* aggs, const void* dout, void* const* daggs,
