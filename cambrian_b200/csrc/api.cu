@@ -148,6 +148,9 @@ int attn_decode_paged_launch(const void*, long long, const void*, const void*, c
                              cudaStream_t);
 int paged_kv_gather_launch(const void*, const void*, const float*, const float*, int, const int*, int, int, int, int, int,
                            long long, void*, void*, long long, cudaStream_t);
+long long sample_tokens_workspace_floats(int, int);
+int sample_tokens_launch(const float*, long long, int, int, const float*, const int*, const float*, const uint64_t*,
+                         const int64_t*, int64_t*, float*, long long, cudaStream_t);
 
 }  // namespace cb
 
@@ -513,6 +516,13 @@ int cb_paged_kv_gather(const void* k_pages, const void* v_pages, const float* k_
                        void* out_k, void* out_v, int64_t out_ld, void* stream) {
   return cb::paged_kv_gather_launch(k_pages, v_pages, k_scales, v_scales, fp8, block_table_row, nkv, hd, page_size,
                                     num_pages, max_pages, P, out_k, out_v, out_ld, ST(stream));
+}
+int64_t cb_sample_tokens_workspace_floats(int rows, int V) { return cb::sample_tokens_workspace_floats(rows, V); }
+int cb_sample_tokens(const float* logits, int64_t ld, int rows, int V, const float* temperature, const int* top_k,
+                     const float* top_p, const uint64_t* seed, const int64_t* step, int64_t* out, float* workspace,
+                     int64_t workspace_floats, void* stream) {
+  return cb::sample_tokens_launch(logits, ld, rows, V, temperature, top_k, top_p, seed, step, out, workspace,
+                                  workspace_floats, ST(stream));
 }
 
 }  // extern "C"

@@ -3,15 +3,35 @@ reference's callers use (cambrian_llama.py:437-483 forwards **kwargs to it; call
 cambrian/serve/model_worker.py:177-187, eval/eval/*/*_eval.py): greedy / temperature + top-k + top-p sampling, EOS and
 user `stopping_criteria`, `streamer`, `max_new_tokens` / `max_length`.
 
-Every keyword is either honoured or rejected with an exception naming it — nothing is silently dropped.  The per-step
-work here is O(batch x vocab) elementwise/sort on the fp32 logits of ONE position (torch ops: plumbing around the decoder
-kernels, which do the O(parameters) work)."""
+Every keyword is either honoured or rejected with an exception naming it — nothing is silently dropped.
+
+Sampling (`do_sample=True`) on CUDA logits runs one kernel, `ops.sample_tokens` (csrc/sample.cu), for all rows of a step;
+`generate()` runs it inside its decode CUDA graph and the server (serving.py) inside each bucket's graph.  The rule:
+  * scores s = logits when temperature == 1, else logits / temperature (IEEE division);
+  * top-k (0 < top_k < V): keep s_i >= the k-th largest score, ties kept (the set `warp_logits` keeps);
+  * top-p (< 1): over the kept scores, keep i iff the softmax mass of the kept scores strictly greater than s_i is below
+    top_p.  The mass is exp(s - max) in fp32, rounded to an integer multiple of 2^-40 and summed exactly, so no summation
+    order enters.  This is HF's rule (sorted ascending, `cumsum <= 1 - top_p` removed) restated, except that a tie at the
+    boundary is kept whole where HF's unstable sort keeps an arbitrary part of it;
+  * draw: the exponential race that torch.multinomial uses (Gumbel-max): the kept i with the largest s_i - log(-log u_i),
+    the lowest index on a tie, where u_i comes from Philox4x32-10 keyed by the row's 64-bit seed at counter
+    (i >> 2, step) and has 23 random bits, strictly inside (0, 1).
+  * seeds: one 64-bit seed S per generate() call, drawn from `generator` (or the default generator of the logits' device)
+    at the first sampled token; row b uses S + b, and token t of a row (t = 0 for the prefill's token) uses step t.  A
+    served request gets the seed row 0 of a solo generate() with the same generator gets.
+So a row's token is a function of its logits, its parameters, its seed and its step alone: the same generator gives the
+same tokens run after run, whatever rows are sampled beside it.  These are not the tokens torch.multinomial's stream
+drew for the same generator before this kernel existed; the distribution is the same warped softmax.
+
+CPU logits keep the torch path: `warp_logits` (HF's warpers) and torch.multinomial with `generator`."""
 from __future__ import annotations
 
 from dataclasses import dataclass, field
 from typing import Callable, List, Optional
 
 import torch
+
+from . import ops
 
 # keywords of HF generate that only make sense with features this path does not implement: rejected when they would
 # change the result, accepted when they carry their neutral value
@@ -38,6 +58,8 @@ class GenerationArgs:
     stopping_criteria: List[Callable] = field(default_factory=list)
     streamer: Optional[object] = None
     generator: Optional[torch.Generator] = None
+    seed: Optional[int] = None  # the sampling seed S, drawn at the first sampled token (draw_seed)
+    step: int = 0               # the index of the next sampled token of the eager loop
 
     @classmethod
     def from_kwargs(cls, model, prompt_len: int, kwargs: dict):
@@ -109,11 +131,41 @@ def warp_logits(logits: torch.Tensor, temperature: float, top_k: int, top_p: flo
     return scores
 
 
+def draw_seed(args: GenerationArgs, device) -> int:
+    """The call's 64-bit sampling seed S, drawn once from args.generator (or the default generator of `device`)."""
+    if args.seed is None:
+        g = args.generator
+        lo, hi = torch.randint(0, 1 << 32, (2,), generator=g, device=g.device if g is not None else device).tolist()
+        args.seed = lo | hi << 32
+    return args.seed
+
+
+def as_int64(v: int) -> int:
+    """A uint64 value as the int64 with the same bits (the seed buffers are int64 tensors)."""
+    v &= (1 << 64) - 1
+    return v - (1 << 64) if v >= 1 << 63 else v
+
+
+def sampling_params(args: GenerationArgs, rows: int, device):
+    """(temperature, top_k, top_p, seed, step) device tensors of ops.sample_tokens for `rows` rows of one call: seed
+    S + b for row b, step args.step."""
+    S = draw_seed(args, device)
+    return (torch.full((rows,), args.temperature, dtype=torch.float32, device=device),
+            torch.full((rows,), min(args.top_k, (1 << 31) - 1), dtype=torch.int32, device=device),
+            torch.full((rows,), args.top_p, dtype=torch.float32, device=device),
+            torch.tensor([as_int64(S + b) for b in range(rows)], dtype=torch.int64, device=device),
+            torch.full((rows,), args.step, dtype=torch.int64, device=device))
+
+
 def next_tokens(logits: torch.Tensor, args: GenerationArgs) -> torch.Tensor:
     if not args.do_sample:
         return logits.argmax(-1)
-    probs = warp_logits(logits, args.temperature, args.top_k, args.top_p).softmax(-1)
-    return torch.multinomial(probs, 1, generator=args.generator).squeeze(-1)
+    if not logits.is_cuda:
+        probs = warp_logits(logits, args.temperature, args.top_k, args.top_p).softmax(-1)
+        return torch.multinomial(probs, 1, generator=args.generator).squeeze(-1)
+    tok = ops.sample_tokens(logits, *sampling_params(args, logits.shape[0], logits.device))
+    args.step += 1
+    return tok
 
 
 def should_stop(args: GenerationArgs, generated: torch.Tensor, scores, done: torch.Tensor) -> torch.Tensor:

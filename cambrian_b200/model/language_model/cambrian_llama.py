@@ -628,7 +628,7 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
         check_stop = bool(args.eos_token_ids or args.stopping_criteria)
         if args.streamer is not None:
             args.streamer.put(torch.empty((B, 0), dtype=torch.long))     # HF streams the (here: empty) prompt ids first
-        if (_DECODE_GRAPH and not args.do_sample and z3 is None and max_new > 2 and h_last.is_cuda
+        if (_DECODE_GRAPH and z3 is None and max_new > 2 and h_last.is_cuda
                 and not getattr(self.config, "disable_decode_graph", False)):
             toks = self._generate_graphed(args, cache, h_last, next_pos, S0, max_new, check_stop)
             self.train(was_training)
@@ -699,12 +699,14 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
         return args, cache, h_last, next_pos, S0
 
     def _generate_graphed(self, args, cache, h_last, next_pos, S0, max_new, check_stop):
-        """Greedy decoding with ONE CUDA graph per generate() call: a decode step is ~290 kernel launches whose device time
+        """Decoding with ONE CUDA graph per generate() call: a decode step is ~290 kernel launches whose device time
         (weight streaming, a few ms) is far below the cost of enqueueing them one by one from Python, so the step is captured
         once — static shapes: token / position /
         cache-slot / validity mask live in device buffers that the captured kernels advance themselves — and replayed per
-        token.  EOS / stopping criteria are evaluated between replays on the host exactly as in the eager loop."""
-        from ...generation import should_stop
+        token.  EOS / stopping criteria are evaluated between replays on the host exactly as in the eager loop.  Greedy
+        decoding takes the argmax; sampling runs ops.sample_tokens on per-row parameter buffers and a step buffer that
+        the graph advances, so it draws the tokens the eager loop's next_tokens draws."""
+        from ...generation import sampling_params, should_stop
         B = h_last.shape[0]
         dev = h_last.device
         pad = args.pad_token_id
@@ -715,10 +717,18 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
         logits_buf = torch.empty((B, self.lm_head.weight.shape[0]), dtype=torch.float32, device=dev)
         cache.slot = torch.full((1,), cache.length, dtype=torch.long, device=dev)
         window = self.attention_window()
+        if args.do_sample:
+            *params, step_buf = sampling_params(args, B, dev)
+            samp_buf = torch.empty(B, dtype=torch.long, device=dev)
+
+        def pick(logits):
+            if not args.do_sample:
+                return logits.argmax(-1)
+            return ops.sample_tokens(logits, *params, step_buf, out=samp_buf)
 
         def step():
             ops.gemm(h_buf, self.lm_head.weight, out=logits_buf)                                 # fp32 logits (:409)
-            nxt = logits_buf.argmax(-1)
+            nxt = pick(logits_buf)
             tok_buf.copy_(torch.where(done_buf, torch.full_like(nxt, pad), nxt))
             cache.kmask.index_fill_(1, cache.slot, True)
             if window:
@@ -730,30 +740,33 @@ class CambrianLlamaForCausalLM(CambrianPreTrainedModel, CambrianMetaForCausalLM)
             h_buf.copy_(out.last_hidden_state[:, 0])
             pos_buf.add_(1)
             cache.slot.add_(1)
+            if args.do_sample:
+                step_buf.add_(1)
 
         # slots beyond the prompt start invalid; each step validates the one it writes
         cache.kmask[:, S0:] = False
         if window:
             cache.kmask[:, :max(0, S0 - window)] = False    # already outside the first step's window
-        snap = (h_buf.clone(), pos_buf.clone(), cache.slot.clone(), cache.kmask.clone())
+        state = (h_buf, pos_buf, cache.slot, cache.kmask) + ((step_buf,) if args.do_sample else ())
+        snap = tuple(t.clone() for t in state)
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):                      # warm-up outside capture (lazy kernel attributes, allocator)
             step()
         torch.cuda.current_stream().wait_stream(side)
-        for buf, s0 in zip((h_buf, pos_buf, cache.slot, cache.kmask), snap):
+        for buf, s0 in zip(state, snap):
             buf.copy_(s0)                                  # the warm-up step advanced the state: rewind (K/V slot S0 is
         graph = torch.cuda.CUDAGraph()                     # simply rewritten with the same values)
         with torch.cuda.graph(graph):
             step()
-        for buf, s0 in zip((h_buf, pos_buf, cache.slot, cache.kmask), snap):
+        for buf, s0 in zip(state, snap):
             buf.copy_(s0)
         tokens = []
         for i in range(max_new):
             if i + 1 == max_new:
-                # the last token needs no further decoder pass: logits -> argmax only
+                # the last token needs no further decoder pass: logits -> argmax or a draw at step i (step_buf) only
                 logits = ops.gemm(h_buf, self.lm_head.weight, out_dtype=torch.float32)
-                nxt = logits.argmax(-1)
+                nxt = pick(logits)
                 tok = torch.where(done_buf, torch.full_like(nxt, pad), nxt)
             else:
                 graph.replay()

@@ -1210,3 +1210,36 @@ def paged_kv_gather(k_pages, v_pages, k_scales, v_scales, block_table_row, P: in
     check(_lib.load().cb_paged_kv_gather(ptr(k_pages), ptr(v_pages), ptr(k_scales), ptr(v_scales), fp8,
                                          ptr(block_table_row), nkv, hd, page_size, num_pages, block_table_row.shape[0],
                                          int(P), ptr(out_k), ptr(out_v), ld, stream()), "cb_paged_kv_gather")
+
+
+def sample_tokens_workspace(rows: int, V: int, device) -> torch.Tensor:
+    """The fp32 workspace `sample_tokens` needs for up to `rows` rows of V logits (at least one element)."""
+    n = _lib.load().cb_sample_tokens_workspace_floats(int(rows), int(V))
+    return torch.empty(max(int(n), 1), dtype=torch.float32, device=device)
+
+
+def sample_tokens(logits, temperature, top_k, top_p, seed, step, out=None, workspace=None):
+    """One sampled token per row of fp32 logits [rows, V] (unit column stride, any row stride >= V) into out int64
+    [rows], each row under its own temperature (fp32 [rows]), top_k (int32 [rows]; 0 or >= V: off), top_p (fp32 [rows];
+    1: off), seed (int64 [rows], read as uint64) and step (int64 [rows]).  The rule is in generation.py's docstring; a
+    row's token depends only on its logits, parameters, seed and step."""
+    if not logits.is_cuda:
+        raise _lib.CambrianB200Error("cambrian_b200 kernels need CUDA tensors (no CPU fallback)")
+    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1 or logits.shape[0] == 0:
+        raise ValueError("sample_tokens: logits must be fp32 [rows >= 1, V] with unit column stride")
+    rows, V = logits.shape
+    ld = logits.stride(0) if rows > 1 else V
+    for name, t, dt in (("temperature", temperature, torch.float32), ("top_k", top_k, torch.int32),
+                        ("top_p", top_p, torch.float32), ("seed", seed, torch.int64), ("step", step, torch.int64)):
+        if t.dtype != dt or t.shape != (rows,) or not t.is_contiguous() or t.device != logits.device:
+            raise ValueError(f"sample_tokens: {name} must be a contiguous {dt} [{rows}] on {logits.device}")
+    if out is None:
+        out = torch.empty(rows, dtype=torch.int64, device=logits.device)
+    elif out.dtype != torch.int64 or out.shape != (rows,) or not out.is_contiguous() or out.device != logits.device:
+        raise ValueError(f"sample_tokens: out must be a contiguous int64 [{rows}] on {logits.device}")
+    if workspace is not None and workspace.dtype != torch.float32:
+        raise ValueError("sample_tokens: the workspace must be fp32")
+    check(_lib.load().cb_sample_tokens(ptr(logits), ld, rows, V, ptr(temperature), ptr(top_k), ptr(top_p), ptr(seed),
+                                       ptr(step), ptr(out), ptr(workspace),
+                                       0 if workspace is None else workspace.numel(), stream()), "cb_sample_tokens")
+    return out

@@ -23,8 +23,13 @@ the true length are returned right after it.
 A step (1) prefills the newly admitted requests one at a time through the prefill of `generate()` (towers, SVA, the
 dynamic branch for non-square images), which gives each its first token; (2) packs the running requests into rows
 [0, n), compacting when one retires; (3) runs one decode step for all of them, padded to a bucket of 1, 2, 4, ...
-rows (padding rows are inactive), as one CUDA graph per bucket captured on first use; (4) samples per request;
-(5) applies EOS and stopping criteria, retires and streams.  Graph and eager (`use_graph=False`) steps run the same
+rows (padding rows are inactive), as one CUDA graph per bucket captured on first use; (4) picks each row's token: the
+argmax for greedy rows and, when a row samples, ops.sample_tokens for all rows with each row's own parameters, seed and
+step in device buffers (written when the row set changes, the steps advanced by the step itself), one torch.where
+choosing per row, inside the same graph (a bucket has a second graph for steps with sampled rows); (5) applies EOS and
+stopping criteria, retires and streams.  A sampled request's seed is the one row 0 of a solo `generate()` with its
+generator draws (generation.py), drawn at its first token, and its token t uses step t, so its tokens are solo
+`generate()`'s wherever their logits are equal.  Graph and eager (`use_graph=False`) steps run the same
 kernels on the same padded shapes and give bitwise identical tokens.  The paged decode attention's result for a row is
 bitwise independent of the other rows.  The rest of the step is not: the projection and lm_head GEMMs pick their kernel
 by the bucket's row count (ops.gemm: the CUDA-core GEMV up to 8 rows, except wide outputs at 6-8 rows; the tensor-core
@@ -62,7 +67,7 @@ from dataclasses import dataclass, field
 import torch
 
 from . import ops
-from .generation import GenerationArgs, next_tokens, should_stop
+from .generation import GenerationArgs, as_int64, draw_seed, next_tokens, should_stop
 from .kv_fp8 import resolve_cache_dtype
 from .model.cambrian_arch import IMAGE_TOKEN_INDEX
 from .paged_kv import DEFAULT_PAGE_SIZE, ROOT, PagedCacheView, PagedKVPool, check_page_size, pages_for
@@ -125,6 +130,15 @@ class BatchedGenerator:
         self._lens = torch.full((mb,), -1, dtype=torch.int32, device=dev)
         self._table = torch.zeros((mb, mpps), dtype=torch.int32, device=dev)
         self._logits = torch.zeros((mb, V), dtype=torch.float32, device=dev)
+        # per-row sampling parameters (greedy and padding rows: T = 1, top_k = 1, top_p = 1), seed, step and pick
+        self._temp = torch.ones(mb, dtype=torch.float32, device=dev)
+        self._topk = torch.ones(mb, dtype=torch.int32, device=dev)
+        self._topp = torch.ones(mb, dtype=torch.float32, device=dev)
+        self._seed = torch.zeros(mb, dtype=torch.long, device=dev)
+        self._step = torch.zeros(mb, dtype=torch.long, device=dev)
+        self._sample = torch.zeros(mb, dtype=torch.bool, device=dev)
+        self._drawn = torch.zeros(mb, dtype=torch.long, device=dev)
+        self._next = torch.zeros(mb, dtype=torch.long, device=dev)
         self.buckets = sorted({min(1 << i, mb) for i in range(mb.bit_length() + 1)})
         self._graphs = {}
         self._graph_pool = torch.cuda.graph_pool_handle() if self.use_graph else None
@@ -132,7 +146,7 @@ class BatchedGenerator:
         self._active: list[_Request] = []
         self._results = {}
         self._next_rid = 0
-        self._dirty = True           # the row set changed since lens / pos / table were last uploaded
+        self._dirty = True           # the row set changed since lens / pos / table / sampling rows were last uploaded
         q_num = int(getattr(cfg, "image_token_len", 576))
         self._image_extra = q_num + int(q_num ** 0.5) - 1
         self.prefix_cache = bool(prefix_cache)
@@ -366,6 +380,8 @@ class BatchedGenerator:
         if args.streamer is not None:
             args.streamer.put(torch.empty((1, 0), dtype=torch.long))     # HF streams the (here: empty) prompt ids first
         logits = ops.gemm(h_last, self.model.lm_head.weight, out_dtype=torch.float32)
+        if args.do_sample:
+            draw_seed(args, self.device)
         tok = int(next_tokens(logits, args)[0])
         finished = self._emit(r, tok, logits)
         if finished:
@@ -397,36 +413,45 @@ class BatchedGenerator:
     def _bucket(self, n: int) -> int:
         return next(b for b in self.buckets if b >= n)
 
-    def _decode_step(self, nb: int):
-        """One decode step over rows [0, nb): embedding -> layers (paged attention) -> norm -> fp32 logits, then the
-        active rows' lengths and positions advance on the device.  Captured as the bucket's CUDA graph."""
+    def _decode_step(self, nb: int, sample: bool):
+        """One decode step over rows [0, nb): embedding -> layers (paged attention) -> norm -> fp32 logits (with `sample`:
+        then each row's token into _next, sampled or the argmax), then the active rows' lengths, positions and steps
+        advance on the device.  Captured as the bucket's CUDA graph."""
         m = self.model
         view = PagedCacheView(self.pool, self._table[:nb], self._lens[:nb], prefill=False)
         out = m.model(input_ids=self._tok[:nb].view(nb, 1), position_ids=self._pos[:nb], past_key_values=view,
                       use_cache=True)
-        ops.gemm(out.last_hidden_state.view(nb, -1), m.lm_head.weight, out=self._logits[:nb])
+        logits = self._logits[:nb]
+        ops.gemm(out.last_hidden_state.view(nb, -1), m.lm_head.weight, out=logits)
         live = self._lens[:nb] >= 0
+        if sample:
+            ops.sample_tokens(logits, self._temp[:nb], self._topk[:nb], self._topp[:nb], self._seed[:nb], self._step[:nb],
+                              out=self._drawn[:nb])
+            self._next[:nb].copy_(torch.where(self._sample[:nb], self._drawn[:nb], logits.argmax(-1)))
+            self._step[:nb].add_(live.long())
         self._pos[:nb].add_(live.view(nb, 1).long())
         self._lens[:nb].add_(live.int())
 
-    def _graph(self, nb: int):
-        g = self._graphs.get(nb)
+    def _graph(self, nb: int, sample: bool):
+        g = self._graphs.get((nb, sample))
         if g is None:
-            snap = (self._pos.clone(), self._lens.clone())
+            state = (self._pos, self._lens, self._step)
+            snap = tuple(t.clone() for t in state)
             side = torch.cuda.Stream(device=self.device)
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):            # warm-up outside capture (lazy kernel attributes, allocator)
-                self._decode_step(nb)
+                self._decode_step(nb, sample)
             torch.cuda.current_stream().wait_stream(side)
-            # the warm-up advanced lens / pos: rewind (its K / V rows are rewritten with the same values by the replay)
-            self._pos.copy_(snap[0])
-            self._lens.copy_(snap[1])
+            # the warm-up advanced lens / pos / steps: rewind (its K / V rows are rewritten with the same values by the
+            # replay)
+            for t, t0 in zip(state, snap):
+                t.copy_(t0)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, pool=self._graph_pool):
-                self._decode_step(nb)
-            self._pos.copy_(snap[0])
-            self._lens.copy_(snap[1])
-            self._graphs[nb] = g
+                self._decode_step(nb, sample)
+            for t, t0 in zip(state, snap):
+                t.copy_(t0)
+            self._graphs[(nb, sample)] = g
         return g
 
     def _decode(self):
@@ -438,21 +463,30 @@ class BatchedGenerator:
             lens = torch.full((nb,), -1, dtype=torch.int32)
             pos = torch.zeros((nb, 1), dtype=torch.long)
             table = torch.zeros((nb, mpps), dtype=torch.int32)
+            temp, topk, topp = torch.ones(nb), torch.ones(nb, dtype=torch.int32), torch.ones(nb)
+            seed, step = torch.zeros(nb, dtype=torch.long), torch.zeros(nb, dtype=torch.long)
+            samp = torch.zeros(nb, dtype=torch.bool)
             for i, r in enumerate(act):
                 lens[i], pos[i, 0], table[i] = r.length, r.pos, r.table
+                a = r.args
+                if a.do_sample:
+                    temp[i], topk[i], topp[i] = a.temperature, min(a.top_k, (1 << 31) - 1), a.top_p
+                    seed[i], step[i], samp[i] = as_int64(a.seed), len(r.tokens), True
             self._lens[:nb].copy_(lens)
             self._pos[:nb].copy_(pos)
             self._table[:nb].copy_(table)
+            for buf, v in ((self._temp, temp), (self._topk, topk), (self._topp, topp), (self._seed, seed),
+                           (self._step, step), (self._sample, samp)):
+                buf[:nb].copy_(v)
             self._dirty = False
         self._tok[:nb].copy_(torch.tensor([r.tokens[-1] for r in act] + [0] * (nb - n), dtype=torch.long))
+        sample = any(r.args.do_sample for r in act)
         if self.use_graph:
-            self._graph(nb).replay()
+            self._graph(nb, sample).replay()
         else:
-            self._decode_step(nb)
+            self._decode_step(nb, sample)
         logits = self._logits[:n]
-        greedy = logits.argmax(-1)
-        picks = [next_tokens(logits[i:i + 1], r.args)[0] if r.args.do_sample else greedy[i] for i, r in enumerate(act)]
-        toks = torch.stack(picks).tolist()
+        toks = (self._next[:n] if sample else logits.argmax(-1)).tolist()
         events, keep = [], []
         for i, (r, tok) in enumerate(zip(act, toks)):
             r.length += 1

@@ -447,6 +447,26 @@ int cb_paged_kv_gather(const void* k_pages, const void* v_pages, const float* k_
                        const int* block_table_row, int nkv, int hd, int page_size, int num_pages, int max_pages, int64_t P,
                        void* out_k, void* out_v, int64_t out_ld, void* stream);
 
+/* Token sampling for generate(do_sample=True) and the server (cambrian_b200/generation.py states the rule for users):
+ * the reference samples through HF's TemperatureLogitsWarper, TopKLogitsWarper, TopPLogitsWarper and
+ * torch.multinomial (GenerationMixin.generate behind cambrian_llama.py:437-483, serve/model_worker.py:161-187).  One token
+ * per row of fp32 logits (element (b, i) at logits + b * ld + i, ld >= V, V < 2^23) into out int64 [rows], each row under
+ * its own parameters, read on the device so that a CUDA graph replay sees their current values: temperature fp32
+ * [rows], top_k int32 [rows] (0 or >= V: off), top_p fp32 [rows] (>= 1: off), seed uint64 [rows], step int64 [rows].
+ *   scores  s_i = x_i when T == 1, else x_i / T (IEEE division);
+ *   top-k   keep s_i >= the k-th largest score, ties kept;
+ *   top-p   over the kept scores, with m_j = rint(expf(s_j - max) * 2^40) as an exact integer sum: keep i iff
+ *           (double) sum{m_j : s_j > s_i} < (double) top_p * (double) sum{m_j}; the maximum is always kept;
+ *   draw    the kept i with the largest s_i - logf(-logf(u_i)) (lowest index on a tie), u_i = ((w >> 9) + 0.5) * 2^-23
+ *           with w = word i & 3 of Philox4x32-10 at key = seed, counter = (i >> 2, step lo32, step hi32, 0).
+ * A row's token depends only on its logits, parameters, seed and step: bitwise run to run, independent of the other rows
+ * and of the grid (one CTA per row, no float atomics).  The parameter arrays and logits are 4-byte aligned, seed, step
+ * and out 8-byte aligned. */
+int64_t cb_sample_tokens_workspace_floats(int rows, int V);
+int cb_sample_tokens(const float* logits, int64_t ld, int rows, int V, const float* temperature, const int* top_k,
+                     const float* top_p, const uint64_t* seed, const int64_t* step, int64_t* out, float* workspace,
+                     int64_t workspace_floats, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,6 +9,10 @@ prefill, against the weight-streaming floor (bf16 weights / measured HBM bandwid
 does not fit one GPU (--config yi34b: Cambrian-34B-shaped, 60 layers) run.  8-bit takes precedence, as in the loader.
 --kv-fp8 runs every batch twice in the same session, with the bf16 KV cache and then with the FP8 one
 (generate(kv_cache_dtype="fp8"), cambrian_b200/kv_fp8.py), and adds the cache's KVCache.nbytes() to each line.
+--sample times sampled decoding at the model worker's defaults (temperature 0.2, top_p 0.7, HF's top_k 50) in three arms,
+alternated twice per batch: greedy (the anchor), sampled (ops.sample_tokens inside the decode graph) and the earlier
+sampled path (the eager per-token loop with the torch warpers and torch.multinomial, rebuilt here by patching
+generation.next_tokens, so the package keeps no switch for it).
 """
 import argparse
 import json
@@ -36,6 +40,7 @@ def main():
     ap.add_argument("--load-fp8", action="store_true", help="FP8 E4M3 decoder projections (quant_fp8)")
     ap.add_argument("--layers", type=int, default=60, help="decoder layers of --config yi34b")
     ap.add_argument("--kv-fp8", action="store_true", help="each batch with the bf16 and then the FP8 KV cache")
+    ap.add_argument("--sample", action="store_true", help="greedy, sampled and the eager torch-sampled loop, alternated")
     args = ap.parse_args()
     from cambrian_b200 import quant, quant_fp8, quant_int8
     from cambrian_b200.model.language_model.cambrian_llama import CambrianLlamaForCausalLM
@@ -77,16 +82,36 @@ def main():
     model._bench_qstats = qstats
     for B in [int(b) for b in str(args.batch).split(",")]:
         for kv in (("bf16", "fp8") if args.kv_fp8 else (None,)):
-            one_batch(args, model, cfg, dev, B, kv)
+            if args.sample:
+                for _ in range(2):
+                    for arm in ("greedy", "sample", "torch_sample_eager"):
+                        one_batch(args, model, cfg, dev, B, kv, arm)
+            else:
+                one_batch(args, model, cfg, dev, B, kv)
 
 
-def one_batch(args, model, cfg, dev, B, kv=None):
-    from cambrian_b200 import _lib
+def torch_next_tokens(logits, a):
+    """The sampling step before ops.sample_tokens: HF's warpers and torch.multinomial on the device."""
+    from cambrian_b200.generation import warp_logits
+    if not a.do_sample:
+        return logits.argmax(-1)
+    probs = warp_logits(logits, a.temperature, a.top_k, a.top_p).softmax(-1)
+    return torch.multinomial(probs, 1, generator=a.generator).squeeze(-1)
+
+
+def one_batch(args, model, cfg, dev, B, kv=None, arm=None):
+    from cambrian_b200 import _lib, generation
     C = bench.CONFIGS["8b-ddp"] if args.config == "yi34b" else bench.CONFIGS[args.config]
     ids = torch.randint(3, cfg.vocab_size, (B, args.prompt - 599), device=dev)
     ids[:, cfg.image_position] = -200
     images = [torch.randn(B, 3, r, r, device=dev).bfloat16() for r in C["res"]]
     kw = dict(images=images, image_sizes=[(336, 336)] * B, do_sample=False)
+    if arm in ("sample", "torch_sample_eager"):
+        kw.update(do_sample=True, temperature=0.2, top_p=0.7, top_k=50)
+    kernel_next_tokens = generation.next_tokens
+    if arm == "torch_sample_eager":
+        generation.next_tokens = torch_next_tokens
+        cfg.disable_decode_graph = True
     kv_bytes = None
     if kv is not None:
         from cambrian_b200.model.language_model.cambrian_llama import KVCache
@@ -105,10 +130,14 @@ def one_batch(args, model, cfg, dev, B, kv=None):
         torch.cuda.synchronize()
         return e0.elapsed_time(e1), _lib.load().cb_launch_count() - l0, out
 
-    run(2)
-    run(2)
-    t1, l1, _ = run(1)
-    tn, ln, out = run(args.new + 1)
+    try:
+        run(2)
+        run(2)
+        t1, l1, _ = run(1)
+        tn, ln, out = run(args.new + 1)
+    finally:
+        generation.next_tokens = kernel_next_tokens
+        cfg.disable_decode_graph = args.no_graph
     ms_tok = (tn - t1) / args.new
     # weight bytes one decode step streams: decoder layers (bf16, NF4 or int8) + norms + lm_head
     qstats = model._bench_qstats
@@ -131,10 +160,10 @@ def one_batch(args, model, cfg, dev, B, kv=None):
                 a_[1] += 1
         top = [dict(kernel=k, ms_per_token=round(v[0] / 1e3 / args.new, 4), launches_per_token=round(v[1] / args.new, 1))
                for k, v in sorted(agg.items(), key=lambda kv: -kv[1][0])[:14]]
-    print(json.dumps(dict(metric="decode_ms_per_token", value=ms_tok, unit="ms", config=args.config, load_4bit=args.load_4bit and not args.load_8bit,
+    print(json.dumps(dict(metric="decode_ms_per_token", value=ms_tok, unit="ms", arm=arm, config=args.config, load_4bit=args.load_4bit and not args.load_8bit,
                           load_8bit=args.load_8bit, load_fp8=args.load_fp8, kv_cache_dtype=kv, kv_cache_bytes=kv_bytes,
                           batch=B, prompt=args.prompt, new_tokens=args.new, prefill_ms=t1, tokens_per_s=B * 1000.0 / ms_tok,
-                          launches_per_token=(ln - l1) / args.new, decode_graph=not args.no_graph, weight_bytes=weight_bytes,
+                          launches_per_token=(ln - l1) / args.new, decode_graph=not cfg.disable_decode_graph and arm != "torch_sample_eager", weight_bytes=weight_bytes,
                           decoder_nf4_bytes=qstats.get("nf4_bytes") if qstats else None,
                           decoder_int8_bytes=qstats.get("int8_bytes") if qstats else None,
                           decoder_fp8_bytes=qstats.get("fp8_bytes") if qstats else None,

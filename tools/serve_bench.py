@@ -3,7 +3,7 @@
 same seeded request mix, in one session, alternated.
 
     python tools/serve_bench.py [--requests 64] [--max-batch 32] [--rounds 2] [--load-fp8] [--kv-fp8] [--out FILE]
-                                [--prefix-cache] [--mix random|shared]
+                                [--prefix-cache] [--mix random|shared] [--sample]
 
 The mix: every request has one image and a text prompt of 64-448 tokens (at least the config's image position, 91
 for the 8B config; plus the 600-position image span), and
@@ -27,6 +27,11 @@ are each warmed up once on a mix of another seed and then timed alternately, eac
 hits on pages of an earlier one).  Reported per server: generated tokens / s, mean and p90 time to first token (from a
 wave's submit to the request's first token), the hit rate and cached pages; then the gather kernel's time (CUDA events)
 at the mix's hit lengths, with its bytes / s against 3.35 TB/s.
+
+`--sample` serves the random mix three ways on one server, alternated per round: greedy (the anchor), sampled at the
+model worker's defaults (temperature 0.2, top_p 0.7, HF's top_k 50; ops.sample_tokens inside the bucket graph), and the
+same sampled requests through the earlier decode step (the greedy graph, then the torch warpers and torch.multinomial
+once per sampled row), rebuilt here by `torch_rows_decode` so the package keeps no switch for it.
 """
 import argparse
 import json
@@ -327,6 +332,104 @@ def main_shared(args, dev, card, cfg, model, kv):
     return lines
 
 
+def torch_rows_decode(srv):
+    """The server's decode step before ops.sample_tokens: the greedy bucket graph, then the torch sampling path once per
+    sampled row, and a host read of the stacked picks."""
+    from cambrian_b200.generation import warp_logits
+    act = srv._active
+    n = len(act)
+    nb = srv._bucket(n)
+    if srv._dirty:
+        mpps = srv.pool.max_pages_per_seq
+        lens = torch.full((nb,), -1, dtype=torch.int32)
+        pos = torch.zeros((nb, 1), dtype=torch.long)
+        table = torch.zeros((nb, mpps), dtype=torch.int32)
+        for i, r in enumerate(act):
+            lens[i], pos[i, 0], table[i] = r.length, r.pos, r.table
+        srv._lens[:nb].copy_(lens)
+        srv._pos[:nb].copy_(pos)
+        srv._table[:nb].copy_(table)
+        srv._dirty = False
+    srv._tok[:nb].copy_(torch.tensor([r.tokens[-1] for r in act] + [0] * (nb - n), dtype=torch.long))
+    srv._graph(nb, False).replay()
+    logits = srv._logits[:n]
+    greedy = logits.argmax(-1)
+    picks = []
+    for i, r in enumerate(act):
+        a = r.args
+        if a.do_sample:
+            probs = warp_logits(logits[i:i + 1], a.temperature, a.top_k, a.top_p).softmax(-1)
+            picks.append(torch.multinomial(probs, 1, generator=a.generator)[0, 0])
+        else:
+            picks.append(greedy[i])
+    toks = torch.stack(picks).tolist()
+    events, keep = [], []
+    for i, (r, tok) in enumerate(zip(act, toks)):
+        r.length += 1
+        r.pos += 1
+        finished = srv._emit(r, tok, logits[i:i + 1])
+        if finished:
+            srv._retire(r)
+        else:
+            keep.append(r)
+        events.append((r.rid, tok, finished))
+    if len(keep) != n:
+        srv._active = keep
+        srv._dirty = True
+    return events
+
+
+def main_sample(args, dev, card, cfg, model, kv):
+    reqs = request_mix(cfg, args.requests, args.seed, dev)
+    n_tokens = sum(r["new"] for r in reqs)
+    srv = make_server(model, args, kv)
+    kernel_decode = srv._decode
+
+    def torch_decode():
+        nb = srv._bucket(len(srv._active))
+        t0 = time.perf_counter()
+        ev = torch_rows_decode(srv)
+        srv.lat.setdefault(nb, []).append((time.perf_counter() - t0) * 1e3)
+        return ev
+
+    def run(way):
+        srv._decode = torch_decode if way == "torch_per_row" else kernel_decode
+        samp = {} if way == "greedy" else dict(do_sample=True, temperature=0.2, top_p=0.7, top_k=50)
+        rids = [srv.submit(r["ids"], images=r["images"], image_sizes=[(336, 336)], max_new_tokens=r["new"],
+                           eos_token_id=None, generator=torch.Generator(device=dev).manual_seed(i) if samp else None,
+                           **samp) for i, r in enumerate(reqs)]
+        outs = srv.run()
+        return [outs[i].tolist() for i in rids]
+
+    warm = reqs[:min(len(reqs), args.max_batch)]
+    for way in ("greedy", "sample", "torch_per_row"):          # warm-up: pool, both graphs of every bucket, allocator
+        srv._decode = torch_decode if way == "torch_per_row" else kernel_decode
+        for i, r in enumerate(warm):
+            srv.submit(r["ids"], images=r["images"], image_sizes=[(336, 336)], max_new_tokens=r["new"], eos_token_id=None,
+                       **({} if way == "greedy" else dict(do_sample=True, temperature=0.2, top_p=0.7,
+                                                          generator=torch.Generator(device=dev).manual_seed(i))))
+        srv.run()
+    lines, toks = [], {}
+    for rnd in range(args.rounds):
+        for way in ("greedy", "sample", "torch_per_row"):
+            srv.lat = {}
+            out, wall, peak = timed(lambda: run(way))
+            toks.setdefault(way, []).append(out)
+            steps = [x for v in srv.lat.values() for x in v]
+            line = dict(way=way, mix="random", round=rnd, requests=len(reqs), generated_tokens=n_tokens, wall_s=wall,
+                        tokens_per_s=n_tokens / wall,
+                        decode_step_ms_mean=sum(steps) / len(steps) if steps else None, peak_alloc_bytes=peak,
+                        kv_cache_dtype=kv, load_fp8=args.load_fp8, max_batch=args.max_batch, card=card)
+            lines.append(line)
+            print(json.dumps(line), flush=True)
+    summary = dict(metric="serve_sample_summary", card=card,
+                   sampled_tokens_reproduce_across_rounds=all(t == toks["sample"][0] for t in toks["sample"]),
+                   greedy_tokens_reproduce_across_rounds=all(t == toks["greedy"][0] for t in toks["greedy"]))
+    lines.append(summary)
+    print(json.dumps(summary), flush=True)
+    return lines
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--requests", type=int, default=64)
@@ -340,6 +443,8 @@ def main():
     ap.add_argument("--prefix-cache", action="store_true", help="serve the random mix with prefix_cache=True")
     ap.add_argument("--mix", choices=("random", "shared"), default="random",
                     help="shared: the prefix cache's workload, with and without the cache (module docstring)")
+    ap.add_argument("--sample", action="store_true",
+                    help="greedy, sampled and the per-row torch-sampled decode step, alternated (module docstring)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("serve_bench.py measures on a GPU; none is visible")
@@ -348,8 +453,8 @@ def main():
     card = card_info()
     cfg, model = build_model(args, dev)
     kv = "fp8" if args.kv_fp8 else "bf16"
-    if args.mix == "shared":
-        lines = main_shared(args, dev, card, cfg, model, kv)
+    if args.mix == "shared" or args.sample:
+        lines = (main_sample if args.sample else main_shared)(args, dev, card, cfg, model, kv)
         if args.out:
             with open(args.out, "w") as f:
                 for ln in lines:
